@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — tokens/s + acceptance rate of self-speculative decoding (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 A STEP is one full generation: a 128-id synthetic prompt -> a 512-token greedy continuation,
 Llama-2-7B architecture, random-init weights (seeded), exit_layer 8, num_speculations 6 —
@@ -17,9 +17,13 @@ times it (self_speculation/generator_base.py:107-129).
            independent replicas serving different prompts (weak scaling, no data-path
            collective); `--tp` instead shards ONE model tensor-parallel over the N GPUs.
 
-`--impl reference` times the reference algorithm's CPU implementation (the oracle port of
-/root/reference/self_speculation/*, which cannot travel to the GPU box) on the host cores, on a
-bounded sample of the same workload.
+`--impl reference` times the reference algorithm's CPU implementation (the oracle port of the
+original project's self_speculation/*) on the host cores, on a bounded sample of the same workload.
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed generation returned to its
+caller as float64 .npy files: `tokens.npy` (the generated token ids), `rounds.npy` (one row per
+speculation round: drafted, matched, emitted) and `acceptance_rate.npy`.  Weights and prompts are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -61,11 +65,13 @@ def parse_args():
     ap.add_argument("--cpu-max-steps", type=int, default=0, help="reference arm: tokens per step")
     ap.add_argument("--cpu-budget", type=float, default=300.0,
                     help="reference arm: seconds of CPU time the K timed generations may take in total")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed generation to DIR/<name>.npy")
     return ap.parse_args()
 
 
 # --------------------------------------------------------------------------------------------
-# clocks: sample nvidia-smi DURING the timed region (B200_PROFILING.md "clocks line")
+# clocks: sample nvidia-smi DURING the timed region
 # --------------------------------------------------------------------------------------------
 class ClockSampler:
     QUERY = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -130,7 +136,7 @@ def measured_peaks():
                 return float(json.load(f)["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "fallback (H100 SXM data sheet)"
 
 
 # --------------------------------------------------------------------------------------------
@@ -357,13 +363,13 @@ class Watchdog:
 def measure_generations(strat, eng, model, prompts, gcfg, args, eos, first, count, e2e=False):
     """`count` generations starting at prompt index `first`, device-timed: CUDA events on the
     engine's stream around prefill and every round, inputs already resident."""
-    out = dict(tokens=0, dev_ms=0.0, bytes=0.0, accs=[], streams=[])
+    out = dict(tokens=0, dev_ms=0.0, bytes=0.0, accs=[], streams=[], last_rounds=[])
     for i in range(count):
         prompt = prompts[(first + i) % len(prompts)]
         eng.begin(exit_layer=gcfg.exit_layer, max_steps=gcfg.max_steps, eos_token_ids=eos)
         eng.prefill(prompt)
         ms = eng.last_device_ms
-        toks, matches, drafted = [], 0, 0
+        toks, matches, drafted, rounds = [], 0, 0, []
         while len(toks) < gcfg.max_steps:
             d = min(gcfg.num_speculations, gcfg.max_steps - len(toks) - 1)
             ctx = eng.kv_len
@@ -373,6 +379,7 @@ def measure_generations(strat, eng, model, prompts, gcfg, args, eos, first, coun
             toks += r.emitted
             matches += r.n_matches
             drafted += r.n_drafted
+            rounds.append((r.n_drafted, r.n_matches, len(r.emitted)))
             if eos[0] in toks:
                 toks = toks[: toks.index(eos[0])]
                 break
@@ -380,7 +387,19 @@ def measure_generations(strat, eng, model, prompts, gcfg, args, eos, first, coun
         out["dev_ms"] += ms
         out["accs"].append(matches / max(1, drafted))
         out["streams"].append(toks)
+        out["last_rounds"] = rounds
     return out
+
+
+def dump_outputs(directory, meas):
+    """What the last timed generation handed back: token ids, per-round trace, acceptance rate."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    arrays = {"tokens": np.asarray(meas["streams"][-1], dtype=np.float64),
+              "rounds": np.asarray(meas["last_rounds"], dtype=np.float64).reshape(-1, 3),
+              "acceptance_rate": np.asarray([meas["accs"][-1]], dtype=np.float64)}
+    for name, arr in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), arr)
 
 
 def class_profile(eng, arch, tp, prompts, gcfg, eos, reps=5):
@@ -403,18 +422,6 @@ def class_profile(eng, arch, tp, prompts, gcfg, eos, reps=5):
     return cls_ms, cls_n, wb, reps
 
 
-def ncu_traffic(arch_name, tp, cls):
-    """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture
-    (profiles/r2_ncu_traffic.json, written by tools/ncu_traffic.py from the raw CSV export)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")) as f:
-            tab = json.load(f)
-        ent = tab.get(f"{arch_name}/tp{tp}", {}).get(cls)
-        return float(ent["dram_bytes_per_launch"]) if ent else None
-    except Exception:
-        return None
-
-
 def roofline_block(args, arch, tp, eng, prompts, gcfg, eos, meas, peak, peak_kind):
     cls_ms, cls_n, wb, reps = class_profile(eng, arch, tp, prompts, gcfg, eos)
     gemm_bytes = sum(wb[k] * cls_n[k] for k in wb)
@@ -430,11 +437,9 @@ def roofline_block(args, arch, tp, eng, prompts, gcfg, eos, meas, peak, peak_kin
             "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
             "peak_source": f"MEASURED_PEAKS.json hbm_gbs ({peak_kind})",
             "bytes_per_launch": wb[dom], "avg_launch_us": dom_us,
-            "traffic": ncu_traffic(args.arch, tp, dom),
             "how": "algorithmic bytes (packed weight bytes of the GEMM) / mean CUDA-event duration of "
                    "its launches in eager rounds on the engine stream (includes launch gaps that graph "
-                   "replay + PDL hide); traffic = dram__bytes_read.sum + dram__bytes_write.sum per launch "
-                   "from the ncu capture under profiles/ (null when no capture of this config is committed)",
+                   "replay + PDL hide)",
             "all_gemm_launches": {"achieved": gemm_bytes / (gemm_ms * 1e-3) / 1e9,
                                   "frac": gemm_bytes / (gemm_ms * 1e-3) / 1e9 / peak,
                                   "launches_per_round": gemm_launches / reps},
@@ -652,6 +657,8 @@ def run_b200_arm(args):
     dog.note = "timed region"
     meas = measure_generations(strat, eng, model, my_prompts, gcfg, args, eos, args.warmup, args.steps, e2e=False)
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, meas)
     launches = eng.launch_count - launches0
     # e2e leg through the plug-in call (wall clock, host ids in / host ids out, every copy and the
     # per-round sync inside the region)
@@ -722,7 +729,7 @@ def run_b200_arm(args):
         "config": {"workload": workload_string(args),
                    "parallelism": f"tp{tp}" if tp > 1 else ("single-gpu" if world == 1 else f"replicas{world}"),
                    **({"tp_collectives": tp_collectives_name()} if tp > 1 else {}),
-                   "l2": "inputs_exceed_l2 (weights 13.5 GB >> 126 MB L2)",
+                   "l2": "inputs_exceed_l2 (weights 13.5 GB >> 50 MB L2)",
                    "step": "one full generation (prefill + rounds)"},
         "clocks": clocks,
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": 4 * args.prompt_len,
@@ -849,7 +856,7 @@ def single_gpu_extras(args, arch, strat, eng, model, prompts, eos, extra):
                                                "hbm_gbs": nb / (ms * 1e-3) / 1e9}
     except Exception as exc:  # pragma: no cover
         extra["autoregressive_same_engine"] = {"error": repr(exc)}
-    # prefill alone (tcgen05 GEMM path): device time of lsk_prefill for 128 and 1024 prompt ids
+    # prefill alone (wgmma GEMM path): device time of lsk_prefill for 128 and 1024 prompt ids
     try:
         pf = {}
         for n in (128, 1024):

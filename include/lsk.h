@@ -1,5 +1,5 @@
 /*
- * lsk.h — C ABI of the B200-native LayerSkip self-speculative decoding engine (liblsk.so).
+ * lsk.h — C ABI of the H100-native LayerSkip self-speculative decoding engine (liblsk.so).
  *
  * The reference (facebookresearch/LayerSkip) has NO FFI: its hot path is Python calling
  * HuggingFace modules.  This ABI is what a binding for that path would bind; each entry point
@@ -36,7 +36,7 @@ typedef enum {
 #define LSK_FLAG_KEEP_LOGITS 1u  /* also store fp32 logits (needed for sampling / debug reads) */
 #define LSK_FLAG_NO_PDL 2u       /* disable programmatic dependent launch                    */
 #define LSK_FLAG_NO_GRAPH 4u     /* launch kernels eagerly instead of replaying CUDA graphs  */
-#define LSK_FLAG_NO_PREFILL_TC 8u /* keep only the decode-layout weights: the prompt pass runs 16 rows at a time on the decode kernels instead of 128 rows at a time on tcgen05 (saves the second, canonical-layout weight copy) */
+#define LSK_FLAG_NO_PREFILL_TC 8u /* keep only the decode-layout weights: the prompt pass runs 16 rows at a time on the decode kernels instead of 128 rows at a time on wgmma (saves the second, canonical-layout weight copy) */
 #define LSK_FLAG_TP_NCCL 16u     /* tp_size > 1: use NCCL all-reduce instead of the one-shot kernels over peer-mapped HBM */
 
 /* Llama architecture + engine sizing.  Replaces what the reference reads off the HF model
@@ -230,7 +230,7 @@ int lsk_test_gemm(const void* packed_dev, int64_t n, int64_t k, const void* x_bf
 int lsk_test_attn(const void* q_dev, const void* k_dev, const void* v_dev, int32_t n_heads,
                   int32_t n_kv_heads, int32_t head_dim, int32_t ctx, int32_t m, int32_t n_splits,
                   const int32_t* page_perm_host, void* out_dev, int32_t iters, float* avg_ms_out);
-/* tcgen05 LM head (csrc/lmhead_tc.cuh, opt-in): logits[m, n] = rmsnorm(x)[m, :] . W[n, :] with
+/* wgmma LM head (csrc/lmhead_tc.cuh, opt-in): logits[m, n] = rmsnorm(x)[m, :] . W[n, :] with
  * W natural bf16 [n, k], x fp32 [m, k], norm_w bf16 [k]; writes fp32 logits [m, n] and per row the
  * arg-max (lowest index wins).  All pointers are device pointers. */
 int lsk_test_lmhead_tc(const void* w_bf16_dev, int64_t n, int64_t k, const float* x_f32_dev,

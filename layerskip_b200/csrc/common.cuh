@@ -1,4 +1,4 @@
-// common.cuh — device helpers shared by the sm_100a kernels of liblsk.
+// common.cuh — device helpers shared by the sm_90a kernels of liblsk.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -117,12 +117,12 @@ __host__ __device__ __forceinline__ size_t kv_elem_offset(int hd, int page, int 
 }
 
 // ---------------------------------------------------------------------------------------
-// K-major SWIZZLE_128B operand layout of the tcgen05 prefill GEMM (prefill_tc.cuh): stages of
+// K-major SWIZZLE_128B operand layout of the wgmma prefill GEMM (prefill_tc.cuh): stages of
 // 128 rows x 64 k (16 KiB); a row's 64 k (128 bytes) are contiguous, rows 128 bytes apart, and
 // inside every 8-row / 1 KiB atom the 16-byte chunks are XOR-swizzled with the row index — the
 // layout a TMA tensor copy with CU_TENSOR_MAP_SWIZZLE_128B would produce, written here directly
-// by the producing kernels so that plain 1-D bulk copies can move it.  (The SWIZZLE_NONE
-// core-matrix layout of round 1 ran the tensor pipe at ~1/4 rate: bank conflicts on operand fetch.)
+// by the producing kernels so that plain 1-D bulk copies can move it (the swizzle keeps the tensor
+// core's operand fetches free of shared-memory bank conflicts).
 // Byte offset of element (row < 128, k):
 // ---------------------------------------------------------------------------------------
 constexpr int kCanonStageBytes = 128 * 64 * 2;

@@ -1,4 +1,4 @@
-// engine.cu — liblsk: C ABI (include/lsk.h) + host-side orchestration of the sm_100a kernels.
+// engine.cu — liblsk: C ABI (include/lsk.h) + host-side orchestration of the sm_90a kernels.
 //
 // The engine owns: packed weights, the paged KV pool, scratch activations, the device-resident
 // generation state, one stream and a cache of CUDA graphs (one per (E, d_req) round shape).
@@ -76,7 +76,7 @@ struct LayerWeights {
   __nv_bfloat16* wd = nullptr;    // packed [hidden, inter_l]
   __nv_bfloat16* ln1 = nullptr;
   __nv_bfloat16* ln2 = nullptr;
-  // tcgen05 prefill (prefill_tc.cuh): second copy in the canonical K-major tile layout
+  // tensor-core prefill (prefill_tc.cuh): second copy in the canonical K-major tile layout
   unsigned char* wqkv_c = nullptr;
   unsigned char* wo_c = nullptr;
   unsigned char* wgu_c = nullptr;
@@ -103,12 +103,12 @@ struct lsk_engine {
   __nv_bfloat16* embed = nullptr;      // [vocab, hidden] natural (replicated)
   __nv_bfloat16* final_norm = nullptr;
   __nv_bfloat16* lm_head = nullptr;    // packed [vocab_l_pad, hidden]
-  // opt-in tcgen05 LM head (lmhead_tc.cuh): a second, canonical-layout copy of the head weights
+  // opt-in wgmma LM head (lmhead_tc.cuh): a second, canonical-layout copy of the head weights
   bool lm_tc = false;
   unsigned char* lm_head_tc = nullptr;   // [lm_tc_tiles][hidden / 64][16 KiB]
   int lm_tc_tiles = 0, lm_tc_grid = 0, lm_tc_stages = 0;
   unsigned globals_loaded = 0;
-  // tcgen05 prefill: 128-token passes (on unless LSK_FLAG_NO_PREFILL_TC / LSK_PREFILL_TC=0)
+  // tensor-core prefill: 128-token passes (on unless LSK_FLAG_NO_PREFILL_TC / LSK_PREFILL_TC=0)
   bool pf_tc = false;
   int pf_stages = 0;
   int kst_h = 0, kst_q = 0, kst_i = 0;          // 64-wide k stages of hidden / q_rows / inter_l
@@ -269,7 +269,7 @@ static GemmSched plan_sched(int NT, int M, int pro, int epi, const GemmPlan& p, 
     best.grid = n_slots < sm_count ? n_slots : sm_count;
     // Tile quantisation: with g CTAs the kernel lasts ceil(n_slots / g) slot-times.  Among the
     // CTA counts that reach the minimum number of waves, take the SMALLEST one that wastes the
-    // fewest slots (e.g. 768 tiles: 128 CTAs x 6 instead of 148 CTAs of which 28 run a 6th tile
+    // fewest slots (e.g. 768 tiles: 128 CTAs x 6 instead of 132 CTAs of which 108 run a 6th tile
     // alone) — the TMA ring lets ~85 % of the SMs saturate HBM (LSK_GRID_EVEN=0 disables).
     static const bool even = !(getenv("LSK_GRID_EVEN") && atoi(getenv("LSK_GRID_EVEN")) == 0);
     if (even && fixed_ring == 0 && n_slots > sm_count) {
@@ -324,9 +324,9 @@ static int launch_gemm(lsk_engine* e, const GemmPlan& p, GemmArgs a) {
 // LL lines (flag inside the data), polls theirs and adds the rank-ordered sum to the residual.
 // Peer mode 3: the fence + flag protocol (A/B).  Without peer access: NCCL all-reduce + residual add,
 // timed by its own event pair so that `comm` never reads 0.
-static int ll_grid(int n2) {
+static int ll_grid(int n2, int sm_count) {
   int g = (n2 + kArThreads - 1) / kArThreads;
-  return g < 1 ? 1 : (g > 148 ? 148 : g);      // every CTA resident at once (spin-wait safety)
+  return g < 1 ? 1 : (g > sm_count ? sm_count : g);      // every CTA resident at once (spin-wait safety)
 }
 static int emit_allreduce_resid_nccl(lsk_engine* e, float* buf, float* x, int M) {
   const lsk_config& c = e->cfg;
@@ -360,7 +360,7 @@ static int emit_allreduce_resid(lsk_engine* e, float* x, int M) {
   if (e->peer_ok) {
     e->cur_class = CLS_COMM;
     const int n2 = M * c.hidden / 2;
-    CU(launch(e, tp_allreduce_ll_kernel, dim3(ll_grid(n2)), dim3(kArThreads), 0, e->peer,
+    CU(launch(e, tp_allreduce_ll_kernel, dim3(ll_grid(n2, e->sm_count)), dim3(kArThreads), 0, e->peer,
               (const float*)e->tp_buf, x, n2));
     return LSK_OK;
   }
@@ -391,13 +391,13 @@ static int emit_gemm_push_resid(lsk_engine* e, const GemmPlan& p, GemmArgs a, fl
   else CU(launch(e, gemm_skinny_push_kernel<2>, dim3(sc.grid), dim3(kGemmThreads), sc.smem, a, e->peer));
   e->cur_class = CLS_COMM;
   const int n2 = a.M * c.hidden / 2;
-  CU(launch(e, tp_finish_ll_kernel, dim3(ll_grid(n2)), dim3(kArThreads), 0, e->peer, x, n2));
+  CU(launch(e, tp_finish_ll_kernel, dim3(ll_grid(n2, e->sm_count)), dim3(kArThreads), 0, e->peer, x, n2));
   return LSK_OK;
 }
 
 // Host-side launch plan of the attention kernel (pure host logic; lsk_plan_attention exposes it):
 // split count = engine constant (batch invariance), ring depth as deep as shared memory allows, and a
-// shared-memory floor that gives a one-wave grid a whole SM per CTA (profiles/r2_attention_sweep.md).
+// shared-memory floor that gives a one-wave grid a whole SM per CTA.
 static int attn_default_splits(int sm_count, int kv_heads_local) {
   return std::max(1, std::min(4, sm_count / std::max(1, kv_heads_local)));
 }
@@ -566,7 +566,7 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
 }
 
 // ---------------------------------------------------------------------------------------------
-// prompt chunk of m <= 128 tokens at positions c0 .. c0+m-1 through every layer on the tcgen05
+// prompt chunk of m <= 128 tokens at positions c0 .. c0+m-1 through every layer on the wgmma
 // GEMMs (forward_early + forward_remainder of llama_model_utils.py:213-276 / 363-383 on s = T_p)
 // ---------------------------------------------------------------------------------------------
 template <int EPI>
@@ -940,9 +940,9 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
   e->use_graph = !(c.flags & LSK_FLAG_NO_GRAPH);
   e->keep_logits = (c.flags & LSK_FLAG_KEEP_LOGITS) != 0;
   // tensor-parallel collectives: one-shot kernels over peer-mapped HBM.  Default 2 = the
-  // row-parallel GEMM pushes its tiles to every rank from its own epilogue as LL lines (measured
-  // 7B TP=2: 173 tok/s; 1 = separate LL push + reduce kernel 169; 3 = fence + flag protocol 129;
-  // 0 = NCCL 134 — profiles/r2_tp2_modes.md).  LSK_FLAG_TP_NCCL forces NCCL from the API.
+  // row-parallel GEMM pushes its tiles to every rank from its own epilogue as LL lines; 1 =
+  // separate LL push + reduce kernel; 3 = fence + flag protocol; 0 = NCCL.  LSK_FLAG_TP_NCCL
+  // forces NCCL from the API.
   {
     const char* env = getenv("LSK_TP_ONESHOT");
     const int mode = env ? atoi(env) : ((c.flags & LSK_FLAG_TP_NCCL) ? 0 : 2);
@@ -976,10 +976,9 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
   e->n_pages = (c.max_ctx + kPageTokens - 1) / kPageTokens;
   e->max_pos = e->n_pages * kPageTokens;
   // split-KV factor: a constant of the engine (results are batch-invariant only for a fixed
-  // partition).  Measured (profiles/r2_attention_sweep.md): the kernel is bound by per-SM load
-  // bandwidth and barrier latency, so the best grid is ONE CTA per SM on as many SMs as possible —
-  // splits = floor(SMs / kv heads), at most 4 (7B: 32 heads x 4 splits; an 8-CTA cluster's barrier
-  // and 8-way merge cost more than the extra SMs bring: 16 heads x 8 splits ran 23 us against 15).
+  // partition).  The kernel is bound by per-SM load bandwidth and barrier latency, so the grid is
+  // ONE CTA per SM on as many SMs as possible — splits = floor(SMs / kv heads), at most 4 (7B: 32
+  // heads x 4 splits; an 8-CTA cluster's barrier and 8-way merge cost more than extra SMs bring).
   e->n_splits = c.attn_splits > 0 ? c.attn_splits : attn_default_splits(e->sm_count, e->kv_heads_l);
   if (const char* env = getenv("LSK_ATTN_SPLITS")) e->n_splits = atoi(env);   // clamped to [1, 8] below
   if (const char* env = getenv("LSK_ATTN_STAGES")) e->attn_stages = atoi(env);
@@ -996,7 +995,7 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
   e->lm_cand = e->p_lm.n_tiles < e->sm_count ? e->p_lm.n_tiles : e->sm_count;
   if (const char* env = getenv("LSK_L2_PREFETCH_MB")) e->l2_prefetch_bytes = (size_t)atoi(env) << 20;
   if (getenv("LSK_LMHEAD_TC") && atoi(getenv("LSK_LMHEAD_TC")) != 0) {
-    // tcgen05 LM head: needs hidden % 64 == 0 and the 16-token B operand + a >= 3-stage ring in
+    // wgmma LM head: needs hidden % 64 == 0 and the 16-token B operand + a >= 3-stage ring in
     // shared memory (hidden <= 5120); otherwise stay on the mma.sync kernel, loudly
     int st = kTcMaxStages;
     while (st >= 3 && lmhead_tc_smem_bytes(c.hidden, st) > (size_t)kSmemMax) --st;
@@ -1008,7 +1007,7 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
       e->lm_tc_grid = (e->lm_tc_tiles + waves - 1) / waves;        // even waves
       e->lm_cand = e->lm_tc_grid;
     } else {
-      fprintf(stderr, "[lsk] LSK_LMHEAD_TC ignored: hidden %d does not fit the tcgen05 LM head\n", c.hidden);
+      fprintf(stderr, "[lsk] LSK_LMHEAD_TC ignored: hidden %d does not fit the wgmma LM head\n", c.hidden);
     }
   }
   e->max_rows = plan_sched(2, kMaxRows, PRO_RMS, EPI_QKV, e->p_qkv, e->sm_count).ok ? kMaxRows : 8;
@@ -1252,7 +1251,7 @@ static int pack(lsk_engine* e, const __nv_bfloat16* src, int64_t src_ld, int64_t
   if (K_dst == 0) K_dst = K;
   const int64_t pairs = n_rows * (K / 2);
   int blocks = (int)((pairs + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > e->sm_count * 32) blocks = e->sm_count * 32;
   if (blocks < 1) blocks = 1;
   pack_rows_kernel<<<blocks, 256, 0, e->stream>>>(src, src_ld, row0, col0, n_rows, K, dst, dst_row0, mode, K_dst, e->cfg.head_dim);
   CU(cudaGetLastError());
@@ -1264,7 +1263,7 @@ static int pack_canon(lsk_engine* e, const __nv_bfloat16* src, int64_t src_ld, i
   if (!e->pf_tc) return LSK_OK;
   const int64_t total = n_rows * (K / 8);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > e->sm_count * 32) blocks = e->sm_count * 32;
   if (blocks < 1) blocks = 1;
   pack_canonical_rows_kernel<<<blocks, 256, 0, e->stream>>>(src, src_ld, row0, col0, n_rows, K, dst, dst_row0, mode,
                                                             n_kst, e->cfg.head_dim);
@@ -1304,7 +1303,7 @@ int lsk_load_weights(lsk_engine* e, const lsk_weight_desc* descs, int32_t n) {
         TRY(expect(c.vocab, h));
         TRY(pack(e, src, h, (int64_t)r * e->vocab_l, 0, e->vocab_l, h, e->lm_head, 0, MAP_PLAIN));
         if (e->lm_tc) {
-          pack_canonical_kernel<<<148 * 8, 256, 0, e->stream>>>(src, h, (int64_t)r * e->vocab_l, e->vocab_l, h,
+          pack_canonical_kernel<<<e->sm_count * 8, 256, 0, e->stream>>>(src, h, (int64_t)r * e->vocab_l, e->vocab_l, h,
                                                               reinterpret_cast<uint4*>(e->lm_head_tc), e->lm_tc_tiles);
           CU(cudaGetLastError());
         }
@@ -1428,7 +1427,7 @@ int lsk_prefill(lsk_engine* e, const int32_t* ids, int32_t n) {
   CU(cudaMemcpyAsync(e->d_prompt, ids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
   // ids[0 .. n-2] through every layer; no LM head: the reference discards those logits too
   // (self_speculation_generator.py:177).  Prompts longer than one decode block go through the
-  // tcgen05 GEMMs 128 tokens per weight pass (prefill_tc.cuh), short ones through the decode
+  // wgmma GEMMs 128 tokens per weight pass (prefill_tc.cuh), short ones through the decode
   // kernels in blocks of <= 16 rows.
   if (e->pf_tc && n - 1 > e->max_rows) {
     for (int c0 = 0; c0 < n - 1; c0 += kPfTokens) {
@@ -1712,7 +1711,7 @@ int lsk_test_pack(const void* w, int64_t n, int64_t k, void* packed) {
   if (!w || !packed || n % 16 || k % 32) return fail(LSK_ERR_INVALID, "need n %% 16 == 0 and k %% 32 == 0");
   const int64_t pairs = n * (k / 2);
   int blocks = (int)((pairs + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 4096) blocks = 4096;
   pack_rows_kernel<<<blocks, 256>>>((const __nv_bfloat16*)w, k, 0, 0, n, k, (__nv_bfloat16*)packed, 0, MAP_PLAIN, k, 128);
   CU(cudaGetLastError());
   CU(cudaDeviceSynchronize());
@@ -1810,8 +1809,8 @@ int lsk_test_attn(const void* q, const void* k, const void* v, int32_t n_heads, 
   const int base = ctx - m;
   CU(cudaMemcpyAsync(pt, pth.data(), (size_t)n_pages * 4, cudaMemcpyHostToDevice, tmp.stream));
   CU(cudaMemcpyAsync(len, &base, 4, cudaMemcpyHostToDevice, tmp.stream));
-  paginate_kv_kernel<<<148 * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)k, n_kv_heads, ctx, head_dim, pt, kp);
-  paginate_kv_kernel<<<148 * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)v, n_kv_heads, ctx, head_dim, pt, vp);
+  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)k, n_kv_heads, ctx, head_dim, pt, kp);
+  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)v, n_kv_heads, ctx, head_dim, pt, vp);
   CU(cudaGetLastError());
   AttnArgs a{};
   a.q = (const __nv_bfloat16*)q; a.q_ld = n_heads * kHeadDim;
@@ -1845,15 +1844,15 @@ int lsk_test_attn(const void* q, const void* k, const void* v, int32_t n_heads, 
   return LSK_OK;
 }
 
-// tcgen05 LM head on caller-provided device buffers (unit test / micro-benchmark of lmhead_tc.cuh)
+// wgmma LM head on caller-provided device buffers (unit test / micro-benchmark of lmhead_tc.cuh)
 int lsk_test_lmhead_tc(const void* w, int64_t n, int64_t k, const float* x, const void* norm_w, float eps,
                        int32_t m, float* logits, float* best_val, int32_t* best_idx, int32_t iters,
                        float* avg_ms) {
   if (!w || !x || !norm_w || !best_val || !best_idx || n < 1 || k % kTcStageK || m < 1 || m > kMaxRows)
-    return fail(LSK_ERR_INVALID, "bad tcgen05 LM-head test shape");
+    return fail(LSK_ERR_INVALID, "bad wgmma LM-head test shape");
   int stages = kTcMaxStages;
   while (stages >= 3 && lmhead_tc_smem_bytes((int)k, stages) > (size_t)kSmemMax) --stages;
-  if (stages < 3) return fail(LSK_ERR_INVALID, "hidden %lld does not fit the tcgen05 LM head", (long long)k);
+  if (stages < 3) return fail(LSK_ERR_INVALID, "hidden %lld does not fit the wgmma LM head", (long long)k);
   int dev = 0, sms = 0;
   CU(cudaGetDevice(&dev));
   CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -1866,7 +1865,7 @@ int lsk_test_lmhead_tc(const void* w, int64_t n, int64_t k, const float* x, cons
   CU(cudaMalloc((void**)&canon, (size_t)n_tiles * kTcTileRows * k * 2));
   CU(cudaMalloc((void**)&cval, (size_t)grid * kMaxRows * 4));
   CU(cudaMalloc((void**)&cidx, (size_t)grid * kMaxRows * 4));
-  pack_canonical_kernel<<<148 * 8, 256>>>((const __nv_bfloat16*)w, k, 0, n, k, reinterpret_cast<uint4*>(canon), n_tiles);
+  pack_canonical_kernel<<<sms * 8, 256>>>((const __nv_bfloat16*)w, k, 0, n, k, reinterpret_cast<uint4*>(canon), n_tiles);
   CU(cudaGetLastError());
   CU(cudaFuncSetAttribute(lmhead_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
   LmHeadTcArgs t{};

@@ -3,7 +3,7 @@
 // HBM-bound by construction (arithmetic intensity <= 16 flop/B).  PRE-SHUFFLED weights are
 // streamed by the TMA engine (1-D cp.async.bulk, global -> shared, mbarrier completion) through
 // a multi-stage shared-memory ring: ~100 KB per SM in flight with no L1 miss tracking involved
-// (measured: the LDG path saturates near 45 GB/s per SM, far below HBM / 148).  Consumer warps
+// (a plain LDG path cannot keep enough bytes in flight per SM to reach HBM bandwidth).  Consumer warps
 // lift mma.sync A-fragments out of the ring with conflict-free 128-bit shared loads; the (tiny)
 // activation block is resident in shared memory as the B operand.
 //
@@ -197,7 +197,7 @@ __device__ __forceinline__ void gemm_load_x_bf16(const GemmArgs& a, unsigned cha
   const int nvec = cols >> 3;                // uint4 (8 bf16) per row
   const int zvec = kc_cols >> 3;
   // four rows per step: their loads are issued together (one L2 round trip per step instead of
-  // one per row — at 7 rows the row-by-row loop cost ~3 us of a 14 us kernel, ncu r2)
+  // one per row)
   for (int m0 = 0; m0 < a.xs_rows; m0 += 4) {
     for (int idx = ltid; idx < zvec; idx += nthreads) {
       uint4 v[4];
@@ -344,11 +344,10 @@ __device__ __forceinline__ void gemm_prologue(const GemmArgs& a, const GemmCtx& 
     // RMSNorm of the fp32 residual rows -> bf16 (rounding point of a bf16 HF model:
     // modeling_llama.py:52-70).  n_chunks == 1 here.  Rows are processed FOUR at a time: each thread
     // pulls its <= 4 float4 slices of all four rows into registers at once (one L2 round trip per
-    // group instead of two per row: the row-by-row version spent ~5 us of a 39 us gate/up launch in
-    // this prologue at 7 rows, ncu r2), reduces, and normalises out of registers.
+    // group instead of two per row), reduces, and normalises out of registers.
     // K <= 4864: 2 slices per thread and row -> groups of 4 rows; larger K: 4 slices -> groups of 2.
-    // (Groups of 8 rows were measured: the 64 live registers spill inside the 96-register budget of
-    // the 640-thread CTA and the round got 9 % SLOWER, 7.32 vs 6.70 ms.)
+    // (Groups of 8 rows would need 64 live registers, which spill inside the 96-register budget of
+    // the 640-thread CTA.)
     // K-chunked (n_chunks > 1: 16-row blocks at hidden > 4096): only the statistics here — the SAME
     // reduction as the resident mode, so a row's rstd does not depend on how the block is staged —
     // and gemm_load_x_rms normalises each chunk when the consumers swap it in.

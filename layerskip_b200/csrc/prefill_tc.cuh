@@ -1,4 +1,4 @@
-// prefill_tc.cuh — the prompt pass on the 5th-generation tensor cores (tcgen05 + TMEM).
+// prefill_tc.cuh — the prompt pass on the Hopper tensor cores (wgmma).
 //
 // The reference's prefill is `forward_early` / `forward_remainder` on s = T_p rows
 // (self_speculation/llama_model_utils.py:213-276, 363-383): a real contraction, unlike the decode
@@ -7,26 +7,29 @@
 //
 //     out[tok, f] = sum_k act[tok, k] * W[f, k]          tok < 128 per launch, f = output feature
 //
-// Swap-AB UMMA: the WEIGHTS are the A operand (M = 128 output features per tile), the ACTIVATIONS
-// the B operand (N = 128 tokens), both K-major in the canonical SWIZZLE_NONE core-matrix layout and
+// Swap-AB warpgroup MMA: the WEIGHTS are the A operand (128 output features per tile), the
+// ACTIVATIONS the B operand (N = 128 tokens), both K-major in the SWIZZLE_128B layout below and
 // both streamed by TMA bulk copies (16 KiB per operand per 64-wide k stage) through one shared-
-// memory ring; the accumulator D[128 features x 128 tokens] fp32 lives in TMEM (128 of 512 columns,
-// double-buffered: the epilogue of tile i overlaps the MMAs of tile i+1).  Weights come from HBM
-// once per launch; the activation block (<= 128 x K bf16) is re-read per feature tile from L2.
-// Roofline: 7B layer = 405 MB of weights / 6.5 TB/s = 62 us vs 52 GFLOP / 1.6 PFLOP/s = 33 us:
-// HBM-bound at 128 tokens, i.e. the prompt costs ONE weight pass per 128 tokens instead of eight.
+// memory ring; the fp32 accumulators D[128 features x 128 tokens] live in the registers of the
+// two consumer warpgroups (64 features each: wgmma.m64n128k16, 64 floats per thread).  Weights
+// come from HBM once per launch; the activation block (<= 128 x K bf16) is re-read per feature
+// tile from L2.  A 7B layer at 128 tokens moves 405 MB of weights for 52 GFLOP: HBM-bound on
+// an H100 (the prompt costs ONE weight pass per 128 tokens instead of eight).
 //
-// Roles (192 threads, as lmhead_tc.cuh): warp 0 = TMA producer (one lane), warp 1 = TMEM
-// allocator + single-lane tcgen05.mma issuer, warps 2..5 = epilogue (tcgen05.ld 32x32b: warp w
-// owns TMEM lanes 32 (w % 4) .. + 31 = 32 output features, all 128 token columns).
+// Roles (384 threads, as lmhead_tc.cuh): warp 0 lane 0 = TMA producer, warpgroups 1 and 2 =
+// MMA issue + epilogue straight from the accumulator registers.  The ring keeps streaming while
+// the consumers run the epilogue of a tile.
 //
 // Operand layouts (common.cuh: canon_offset): K-major SWIZZLE_128B — stage (128 rows x 64 k) =
 //   16 KiB, row r at r*128 B, 16-byte chunk c of a row stored at c ^ (r & 7).  Descriptor: layout
-//   type 2 (SWIZZLE_128B), SBO = 1024 B (next 8-row atom), LBO unused (1); one tcgen05.mma eats
-//   K = 16 = 32 bytes of a row: 4 MMAs per stage, start address advancing by 32 B.
+//   type 1 (128-byte swizzle), SBO = 1024 B (next 8-row atom), LBO unused (16 B); one wgmma eats
+//   K = 16 = 32 bytes of a row: 4 MMAs per stage, start address advancing by 32 B.  Consumer
+//   warpgroup g reads A rows 64 g .. 64 g + 63 (8 atoms = 8 KiB into the stage).  Stages must sit
+//   on 1024-byte boundaries (the swizzle pattern is anchored to the address).
 //   Weights: [tile][k stage][16 KiB], packed once with the SAME row permutations as the decode
-//   layout (rotary pairs / gate-up pairs sit 8 rows apart).  Activations: [k stage][16 KiB] with
-//   rows = tokens, written in this layout by the producing kernel.
+//   layout (rotary pairs / gate-up pairs sit 8 rows apart: one accumulator thread holds both rows
+//   of a pair).  Activations: [k stage][16 KiB] with rows = tokens, written in this layout by
+//   the producing kernel.
 //
 // Grid: one CTA per work item wave; a work item = (feature tile, k split).  Row-parallel GEMMs with
 // few feature tiles (O / down projections: hidden / 128 = 32 tiles at 7B) split K so that ~all SMs
@@ -41,7 +44,6 @@ namespace lsk {
 constexpr int kPfTokens = 128;                 // UMMA N: token rows per prefill pass
 constexpr int kPfStageBytes = 2 * kTcStageBytes;   // A stage + B stage
 constexpr int kPfMaxStages = 6;
-constexpr int kPfTmemCols = 256;               // 2 accumulators x 128 token columns
 
 enum { PF_EPI_QKV = 0, PF_EPI_STORE = 2, PF_EPI_SILU = 3 };
 
@@ -71,35 +73,32 @@ struct PrefillGemmArgs {
   int q_rows, kv_rows, n_kv_heads;
 };
 
+// + 1 KiB: the ring is aligned up to 1024 bytes inside the dynamic shared memory
 __host__ __device__ inline size_t prefill_tc_smem_bytes(int n_stages) {
-  return (size_t)kTcHeaderBytes + (size_t)n_stages * kPfStageBytes;
+  return (size_t)kTcHeaderBytes + 1024 + (size_t)n_stages * kPfStageBytes;
 }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor: start address,
-// LBO = 1 (unused for swizzled K-major), SBO = 1024 B, version 1, layout type 2)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-
-__device__ __forceinline__ void tmem_alloc_cols(uint32_t* smem_dst, uint32_t cols) {      // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cols(uint32_t taddr, uint32_t cols) {        // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T (bf16 in, fp32 accumulate, both K-major in shared
+// memory); fragment layout as wgmma_m64n16 (lmhead_tc.cuh), 16 column groups of 8
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
 
 // natural [rows, K] bf16 -> canonical tiles with a row permutation (`mode`: misc_kernels.cuh map_row)
@@ -183,31 +182,23 @@ prefill_gemm_tc_kernel(const PrefillGemmArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem);
   uint64_t* empty_bar = full_bar + kPfMaxStages;
-  uint64_t* tfull_bar = empty_bar + kPfMaxStages;            // [2] accumulator ready
-  uint64_t* tempty_bar = tfull_bar + 2;                      // [2] accumulator drained
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  unsigned char* ring = smem + kTcHeaderBytes;
+  unsigned char* ring = smem + kTcHeaderBytes + ((1024u - (smem_u32(smem) + kTcHeaderBytes) % 1024u) % 1024u);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int NS = a.n_stages;
   const int KS = (EPI == PF_EPI_STORE && a.k_splits > 1) ? a.k_splits : 1;
   const int n_items = a.n_tiles * KS;
 
   if (tid == 0) {
-    for (int s = 0; s < NS; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tfull_bar[b], 1); mbar_init(&tempty_bar[b], 4); }
+    for (int s = 0; s < NS; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kTcConsumerThreads); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc_cols(tmem_slot, kPfTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   pdl_launch_dependents();
   pdl_wait();          // the activations (B operand) are the previous kernel's output
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (tid == 0) {
       // ============================================================ TMA PRODUCER
       uint32_t q = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
@@ -223,127 +214,101 @@ prefill_gemm_tc_kernel(const PrefillGemmArgs a) {
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================================================== MMA ISSUER (one lane)
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(kTcTileRows, kPfTokens);
-      uint32_t q = 0;
-      int it = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
-        const int tile = item / KS, ks = item - tile * KS;
-        const int s_lo = (int)((long long)a.n_kst * ks / KS), s_hi = (int)((long long)a.n_kst * (ks + 1) / KS);
-        (void)tile;
-        const int buf = it & 1;
-        mbar_wait_bounded(&tempty_bar[buf], ((it >> 1) & 1) ^ 1);      // epilogue drained this buffer
-        tc_fence_after();
-        const uint32_t d_addr = tmem_base + (uint32_t)buf * kPfTokens;
-        for (int s = s_lo; s < s_hi; ++s, ++q) {
-          const int st = q % NS;
-          mbar_wait_bounded(&full_bar[st], (q / NS) & 1);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(ring + (size_t)st * kPfStageBytes);
-          const uint32_t b_addr = a_addr + kTcStageBytes;
-#pragma unroll
-          for (int k = 0; k < kTcStageK / 16; ++k) {
-            const uint64_t da = umma_desc_sw128(a_addr + k * 32);
-            const uint64_t db = umma_desc_sw128(b_addr + k * 32);
-            umma_bf16_ss(d_addr, da, db, idesc, (s > s_lo || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[st]);               // frees the ring slot once these MMAs have read it
-        }
-        umma_commit(&tfull_bar[buf]);                // accumulator of this tile complete
-      }
-    }
-  } else {
-    // ================================================================ EPILOGUE (4 warps x 32 features)
-    const int quarter = warp & 3;                    // TMEM lane quarter this warp may access
-    int it = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
-      const int tile = item / KS, ks = item - tile * KS;
-      const int buf = it & 1;
-      mbar_wait_bounded(&tfull_bar[buf], (it >> 1) & 1);
-      tc_fence_after();
-      const int prow = tile * kTcTileRows + quarter * 32 + lane;       // packed output row (feature)
-      const bool valid = prow < a.n_rows;
-      const int r16 = prow & 15;
-#pragma unroll 1
-      for (int c0 = 0; c0 < kPfTokens; c0 += 32) {
-        if (c0 >= a.M) break;                        // warp-uniform: no token rows beyond M
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * kPfTokens + c0), v);
-        if (EPI == PF_EPI_STORE) {
-          float* outp = a.out_f32 + (size_t)ks * kPfTokens * a.out_ld + prow;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int tok = c0 + j;
-            if (tok < a.M && valid) outp[(size_t)tok * a.out_ld] = __uint_as_float(v[j]);
-          }
-        } else if (EPI == PF_EPI_SILU) {
-          // 16-row groups: rows 0..7 gate, rows 8..15 up of the same 8 features (MAP_GATE / MAP_UP)
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float mine = __uint_as_float(v[j]);
-            const float other = __shfl_xor_sync(0xffffffffu, mine, 8);
-            const int tok = c0 + j;
-            if (r16 < 8 && tok < a.M && valid) {
-              const float sg = mine / (1.f + __expf(-mine));
-              const int kidx = (prow >> 4) * 8 + r16;
-              *reinterpret_cast<__nv_bfloat16*>(a.act_canon + canon_offset(tok, kidx)) = __float2bfloat16_rn(sg * other);
-            }
-          }
-        } else {  // PF_EPI_QKV
-          // everything that depends only on the output row is computed once per thread; the RoPE
-          // factors of the 32 tokens are fetched up front (independent loads, one round trip)
-          const int HD = a.head_dim, half = HD >> 1;
-          const bool is_q = prow < a.q_rows, is_k = !is_q && prow < a.q_rows + a.kv_rows;
-          const int rel = is_q ? prow : (is_k ? prow - a.q_rows : prow - a.q_rows - a.kv_rows);
-          const int head = rel / HD, inhead = rel - head * HD;
-          const bool upper = r16 >= 8;                              // upper row of a rotary pair
-          const int d = (inhead >> 4) * 8 + (r16 & 7);              // pair index (q / k rows)
-          const int dd = (is_q || is_k) ? (upper ? d + half : d) : inhead;
-          const float2* __restrict__ rope = a.rope;
-          float2 cs[32];
-          if (is_q || is_k) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int tok = min(c0 + j, a.M - 1);
-              cs[j] = __ldg(rope + (size_t)(a.pos0 + tok) * half + d);
-            }
-          }
-          const int page_lo = a.page_table[(a.pos0 + c0) >> 6];
-          const int page_hi = a.page_table[(a.pos0 + min(c0 + 31, a.M - 1)) >> 6];
-          __nv_bfloat16* __restrict__ qo = a.q_out + head * HD + dd;
-          __nv_bfloat16* __restrict__ pool = is_k ? a.kpool : a.vpool;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float mine = __uint_as_float(v[j]);
-            const float other = __shfl_xor_sync(0xffffffffu, mine, 8);
-            const int tok = c0 + j;
-            if (tok >= a.M || !valid) continue;
-            const int pos = a.pos0 + tok;
-            // lower row of the pair holds x[d] (lo), upper row x[d + half] (hi):
-            //   out_lo = lo cos - hi sin,  out_hi = hi cos + lo sin   (rotate_half, modeling_llama.py:138-168)
-            float outv = mine;
-            if (is_q || is_k) outv = upper ? mine * cs[j].x + other * cs[j].y : mine * cs[j].x - other * cs[j].y;
-            const __nv_bfloat16 ob = __float2bfloat16_rn(outv);
-            if (is_q) {
-              qo[(size_t)tok * a.q_ld] = ob;
-            } else {
-              const int page = ((pos >> 6) == ((a.pos0 + c0) >> 6)) ? page_lo : page_hi;
-              pool[kv_elem_offset(HD, page, a.n_kv_heads, head, pos & 63, dd)] = ob;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[buf]);  // the MMA warp may overwrite this buffer
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc_cols(tmem_base, kPfTmemCols);
+  // ================================================================ CONSUMERS (2 warpgroups x 64 features)
+  const int wg = (warp - 4) >> 2;
+  const int r_lo = ((warp - 4) & 3) * 16 + (lane >> 2);   // accumulator rows r_lo, r_lo + 8 of this warpgroup
+  uint32_t q = 0;
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    const int tile = item / KS, ks = item - tile * KS;
+    const int s_lo = (int)((long long)a.n_kst * ks / KS), s_hi = (int)((long long)a.n_kst * (ks + 1) / KS);
+    float d[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) d[j] = 0.f;
+    for (int s = s_lo; s < s_hi; ++s, ++q) {
+      const int st = q % NS;
+      mbar_wait_bounded(&full_bar[st], (q / NS) & 1);
+      const uint32_t a_addr = smem_u32(ring + (size_t)st * kPfStageBytes) + wg * 8192;
+      const uint32_t b_addr = smem_u32(ring + (size_t)st * kPfStageBytes) + kTcStageBytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kTcStageK / 16; ++k)
+        wgmma_m64n128(d, wgmma_desc(a_addr + k * 32, 16, 1024, 1), wgmma_desc(b_addr + k * 32, 16, 1024, 1),
+                      (s > s_lo || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      if (s > s_lo) {                                 // the previous stage's MMAs are done reading it
+        wgmma_wait<1>();
+        mbar_arrive(&empty_bar[(q - 1) % NS]);
+      }
+    }
+    wgmma_wait<0>();
+    if (s_hi > s_lo) mbar_arrive(&empty_bar[(q - 1) % NS]);
+
+    // d[4 n + c] = (row r_lo, token 8 n + 2 (lane % 4) + c), d[4 n + 2 + c] = (row r_lo + 8, same token):
+    // the lower and upper row of a gate/up or rotary pair are in the same thread
+    const int prow = tile * kTcTileRows + wg * 64 + r_lo;   // packed output row (feature), lower of the pair
+    const bool valid_lo = prow < a.n_rows, valid_hi = prow + 8 < a.n_rows;
+    if (EPI == PF_EPI_STORE) {
+      float* outp = a.out_f32 + (size_t)ks * kPfTokens * a.out_ld + prow;
+#pragma unroll
+      for (int j = 0; j < 64; ++j) {
+        const int tok = 8 * (j >> 2) + 2 * (lane & 3) + (j & 1);
+        const bool hi = (j & 2) != 0;
+        if (tok < a.M && (hi ? valid_hi : valid_lo)) outp[(size_t)tok * a.out_ld + (hi ? 8 : 0)] = d[j];
+      }
+    } else if (EPI == PF_EPI_SILU) {
+      // 16-row groups: rows 0..7 gate, rows 8..15 up of the same 8 features (MAP_GATE / MAP_UP)
+      const int kidx = (prow >> 4) * 8 + (prow & 7);
+#pragma unroll
+      for (int j = 0; j < 64; ++j) {
+        if (j & 2) continue;
+        const int tok = 8 * (j >> 2) + 2 * (lane & 3) + (j & 1);
+        if (tok < a.M && valid_lo) {
+          const float g = d[j], u = d[j + 2];
+          const float sg = g / (1.f + __expf(-g));
+          *reinterpret_cast<__nv_bfloat16*>(a.act_canon + canon_offset(tok, kidx)) = __float2bfloat16_rn(sg * u);
+        }
+      }
+    } else {  // PF_EPI_QKV
+      // a pair never straddles q / k / v or a head (all are multiples of head_dim >= 32 rows)
+      const int HD = a.head_dim, half = HD >> 1;
+      const bool is_q = prow < a.q_rows, is_k = !is_q && prow < a.q_rows + a.kv_rows;
+      const int rel = is_q ? prow : (is_k ? prow - a.q_rows : prow - a.q_rows - a.kv_rows);
+      const int head = rel / HD, inhead = rel - head * HD;
+      const bool rot = is_q || is_k;
+      const int dp = (inhead >> 4) * 8 + (inhead & 7);          // pair index (q / k rows)
+      const int dd_lo = rot ? dp : inhead, dd_hi = rot ? dp + half : inhead + 8;
+      const float2* __restrict__ rope = a.rope;
+      __nv_bfloat16* __restrict__ pool = is_k ? a.kpool : a.vpool;
+#pragma unroll
+      for (int j = 0; j < 64; ++j) {
+        if (j & 2) continue;
+        const int tok = 8 * (j >> 2) + 2 * (lane & 3) + (j & 1);
+        if (tok >= a.M || !valid_lo) continue;
+        const int pos = a.pos0 + tok;
+        // lower row of the pair holds x[d] (lo), upper row x[d + half] (hi):
+        //   out_lo = lo cos - hi sin,  out_hi = hi cos + lo sin   (rotate_half, modeling_llama.py:138-168)
+        const float lo = d[j], hi = d[j + 2];
+        float out_lo = lo, out_hi = hi;
+        if (rot) {
+          const float2 cs = __ldg(rope + (size_t)pos * half + dp);
+          out_lo = lo * cs.x - hi * cs.y;
+          out_hi = hi * cs.x + lo * cs.y;
+        }
+        if (is_q) {
+          __nv_bfloat16* qo = a.q_out + (size_t)tok * a.q_ld + head * HD;
+          qo[dd_lo] = __float2bfloat16_rn(out_lo);
+          qo[dd_hi] = __float2bfloat16_rn(out_hi);
+        } else {
+          const int page = a.page_table[pos >> 6];
+          pool[kv_elem_offset(HD, page, a.n_kv_heads, head, pos & 63, dd_lo)] = __float2bfloat16_rn(out_lo);
+          if (valid_hi) pool[kv_elem_offset(HD, page, a.n_kv_heads, head, pos & 63, dd_hi)] = __float2bfloat16_rn(out_hi);
+        }
+      }
+    }
+  }
 }
 
 }  // namespace lsk

@@ -1,15 +1,13 @@
-// tp_peer.cuh — one-shot collectives over peer-mapped HBM (NVLink 5 / NVSwitch) for the
+// tp_peer.cuh — one-shot collectives over peer-mapped HBM (NVLink / NVSwitch) for the
 // tensor-parallel engine.  This is the DEFAULT data path under tensor parallelism
 // (LSK_TP_ONESHOT selects the protocol, 0 = NCCL; engine.cu: emit_allreduce_resid /
-// emit_gemm_push_resid); the measured comparison is profiles/r2_tp2_modes.md.  The fence + flag
-// protocol described first is round 1's design (mode 3); the LL protocol further down (modes 1 and
-// 2, the default) replaced it after it measured 24 % slower.
+// emit_gemm_push_resid).  The fence + flag protocol described first is mode 3; the LL protocol
+// further down (modes 1 and 2) is the default.
 //
 // Why: a round of the TP engine performs 2 x [(d+1) E + (L-E)] all-reduces of <= 16 x hidden fp32
 // (SURVEY.md §8(e): 176 per round at 13B) plus d+1 arg-max exchanges, every one on the critical
-// path of a batch-1 decode.  At these sizes (8 ... 512 KiB) a collective is pure latency; the
-// measured cost of "row-parallel GEMM -> ncclAllReduce -> residual add" is ~28 us per instance
-// against ~2 us of weight streaming (DESIGN.md §6).  Here every rank owns a small region of HBM
+// path of a batch-1 decode.  At these sizes (8 ... 512 KiB) a collective is pure latency: far
+// more than the few microseconds of weight streaming per instance.  Here every rank owns a small region of HBM
 // that all peers map (CUDA IPC), and ONE kernel per instance
 //     pushes its partial rows into every peer's region (plain stores over NVLink),
 //     raises a flag per (source rank, CTA) with release semantics at system scope,

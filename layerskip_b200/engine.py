@@ -34,13 +34,13 @@ class Engine:
                  attn_splits: int = 0, device: Optional[torch.device] = None,
                  tp_nccl: bool = False, prefill_tc: Optional[bool] = None):
         if not torch.cuda.is_available():
-            raise RuntimeError("layerskip_b200 needs a CUDA device (B200); there is no CPU path")
+            raise RuntimeError("layerskip_b200 needs a CUDA device (H100); there is no CPU path")
         self._lib = _lib.load()
         self.arch = arch
         self.device = torch.device(device) if device is not None else \
             torch.device("cuda", torch.cuda.current_device())
         self.tp_rank, self.tp_size = tp_rank, tp_size
-        # the tcgen05 prompt pass needs a second (canonical-layout) copy of the layer weights: on by
+        # the tensor-core prompt pass needs a second (canonical-layout) copy of the layer weights: on by
         # default, dropped automatically when the two copies would not fit this GPU
         try:
             free_now = torch.cuda.mem_get_info(self.device)[0]
@@ -90,7 +90,8 @@ class Engine:
         # K-chunked normalisation above), else 8
         plan = _lib.lsk_gemm_plan()
         qkv_rows = (arch.heads + 2 * arch.kv_heads) // tp_size * arch.head_dim
-        ok = self._lib.lsk_plan_gemm((qkv_rows + 15) // 16 * 16, arch.hidden, 16, 0, 0, 148, C.byref(plan))
+        sms = torch.cuda.get_device_properties(self.device).multi_processor_count
+        ok = self._lib.lsk_plan_gemm((qkv_rows + 15) // 16 * 16, arch.hidden, 16, 0, 0, sms, C.byref(plan))
         self.max_rows = 16 if (ok == 0 and plan.ok) else 8
 
     # ------------------------------------------------------------------ lifetime

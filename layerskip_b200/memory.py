@@ -1,6 +1,6 @@
 """HBM budget of one engine (per GPU), from the same formulas as the allocations in
 `csrc/engine.cu: create_into` — so a configuration that cannot fit is refused with an explanation
-BEFORE `cudaMalloc` runs out half-way (B200: 180 GB of HBM3e per GPU).
+BEFORE `cudaMalloc` runs out half-way (H100: 80 GB of HBM3 per GPU).
 
 Dominant terms: packed bf16 weights (the per-rank shard under tensor parallelism; embeddings are
 replicated), and the paged KV pool `2 x layers x pages x kv_heads_local x 64 x 128 x 2 B`.
@@ -13,7 +13,8 @@ from .weights import LlamaArch
 
 PAGE_TOKENS = 64
 MAX_ROWS = 16
-HBM_PER_B200 = 180e9
+HBM_PER_GPU = 80e9                  # H100 SXM
+SM_COUNT = 132                      # H100 SXM: one arg-max candidate slot per SM
 
 
 def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling: bool = False,
@@ -30,7 +31,7 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
     per_layer = 2 * ((q_l + 2 * kv_l) * h + h * q_l + 2 * inter_l * h + h * inter_l_pad) + 2 * 2 * h
     weights = L * per_layer
     if prefill_tc and h % 64 == 0:
-        # second, canonical-layout copy of the layer weights for the tcgen05 prompt pass
+        # second, canonical-layout copy of the layer weights for the tensor-core prompt pass
         # (128-row tiles x 64-wide k stages of 16 KiB) + its 128-token activation buffers
         up = lambda x, m: (x + m - 1) // m     # noqa: E731
         t_qkv, t_h, t_gu = up(q_l + 2 * kv_l, 128), up(h, 128), up(2 * inter_l, 128)
@@ -39,7 +40,7 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
     embed = 2 * arch.vocab * h + 2 * h                       # replicated embedding + final norm
     lm_head = 2 * vocab_l_pad * h
     if lm_head_tc:
-        lm_head += 2 * ((vocab_l + 127) // 128 * 128) * h     # canonical-layout copy for tcgen05
+        lm_head += 2 * ((vocab_l + 127) // 128 * 128) * h     # canonical-layout copy for the wgmma head
     n_pages = (max_ctx + PAGE_TOKENS - 1) // PAGE_TOKENS
     max_pos = n_pages * PAGE_TOKENS
     kv_pool = 2 * L * n_pages * (arch.kv_heads // tp_size) * PAGE_TOKENS * arch.head_dim * 2
@@ -49,7 +50,7 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
         + MAX_ROWS * inter_l_pad * 2           # SiLU * up
         + MAX_ROWS * h * 4                     # TP partial sums
         + max_pos * (arch.head_dim // 2) * 8 + max_pos * 4 + n_pages * 4   # RoPE table, prompt ids, page table
-        + 148 * MAX_ROWS * 8 + tp_size * MAX_ROWS * 8)      # arg-max candidates
+        + SM_COUNT * MAX_ROWS * 8 + tp_size * MAX_ROWS * 8)      # arg-max candidates
     if prefill_tc and h % 64 == 0:
         scratch += 6 * 128 * h * 4 + 128 * q_l * 2 + 16384 * (h // 64 + (q_l + 63) // 64 + (inter_l + 63) // 64)
     if keep_logits or sampling:

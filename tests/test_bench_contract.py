@@ -1,9 +1,11 @@
-"""CPU: bench.py's output contract on the arm that runs without a GPU (`--impl reference`):
-exactly ONE line on stdout, valid JSON, every key the driver reads."""
+"""bench.py's output contract: on the arm that runs without a GPU (`--impl reference`) exactly ONE
+line on stdout, valid JSON, every key a caller reads; on the GPU arm, `--dump-outputs`."""
 import json
 import os
 import subprocess
 import sys
+
+import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -42,3 +44,26 @@ def test_usable_cpu_detection_is_sane():
     n = bench.usable_cpus()
     assert 1 <= n <= (os.cpu_count() or 1)
     assert 1 <= bench.cpu_threads() <= 32
+
+
+@pytest.mark.gpu
+def test_dump_outputs_writes_the_last_timed_generation(tmp_path):
+    """`--dump-outputs DIR`: float64 .npy files of what the last timed generation returned to its
+    caller, identical on a second run with the same arguments (seeded weights and prompts)."""
+    import numpy as np
+    args = [sys.executable, os.path.join(ROOT, "bench.py"), "--arch", "tiny-gqa", "--exit-layer", "3",
+            "--num-speculations", "4", "--steps", "2", "--warmup", "1", "--prompt-len", "12",
+            "--max-steps", "32", "--no-extra", "--no-cpu-baseline"]
+    runs = []
+    for i in range(2):
+        out = tmp_path / f"run{i}"
+        proc = subprocess.run(args + ["--dump-outputs", str(out)], capture_output=True, text=True,
+                              timeout=600, cwd=ROOT)
+        assert proc.returncode == 0, proc.stderr[-2000:]
+        assert json.loads(proc.stdout.strip().splitlines()[-1])["steps"] == 2
+        runs.append({n: np.load(out / f"{n}.npy") for n in ("tokens", "rounds", "acceptance_rate")})
+    tokens, rounds = runs[0]["tokens"], runs[0]["rounds"]
+    assert tokens.dtype == np.float64 and 1 <= tokens.size <= 32
+    assert rounds.shape[1] == 3 and rounds[:, 2].sum() >= tokens.size      # emitted before EOS truncation
+    for name in runs[0]:
+        np.testing.assert_array_equal(runs[0][name], runs[1][name])

@@ -253,8 +253,8 @@ def test_unsupported_inputs_fail_loudly(strategies):
                                 logits_processors=[lambda i, s: s])
 
 
-def test_tcgen05_prefill_matches_the_decode_kernel_prefill(monkeypatch):
-    """lsk_prefill through the 128-token tcgen05 GEMMs (csrc/prefill_tc.cuh) vs the same prompt
+def test_wgmma_prefill_matches_the_decode_kernel_prefill(monkeypatch):
+    """lsk_prefill through the 128-token wgmma GEMMs (csrc/prefill_tc.cuh) vs the same prompt
     16 rows at a time through the decode kernels: same K/V rows up to bf16 rounding of different
     accumulation orders, next-step logits within the usual engine-vs-oracle tolerance, same token."""
     from layerskip_b200.engine import Engine

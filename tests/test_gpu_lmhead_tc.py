@@ -1,6 +1,6 @@
-"""GPU: the tcgen05 / TMEM LM head (csrc/lmhead_tc.cuh, LSK_LMHEAD_TC=1).  Executed for the first
-time in round 2: correct, but slower than the mma.sync head at decode widths (3.6 vs 5.7 TB/s at
-7 rows — profiles/r2_unrun_experimental_1gpu.log), so it stays opt-in; these tests keep it honest."""
+"""GPU: the wgmma LM head (csrc/lmhead_tc.cuh, LSK_LMHEAD_TC=1).  It is opt-in (the mma.sync head
+is the default at decode widths); these tests keep it honest.  The test names keep the kernel's
+first implementation (tcgen05) so that their ids stay stable."""
 import pytest
 import torch
 
@@ -38,13 +38,13 @@ def test_tcgen05_lm_head_matches_a_torch_reference(n, k, m):
     assert float((logits - ref).abs().max()) < 2e-2
     assert torch.equal(bi[:m].long(), logits.argmax(-1))        # ties: lowest index, like torch
     assert torch.equal(bv[:m], logits.max(-1).values)
-    print(f"tcgen05 lm head n={n} k={k} m={m}: {ms.value * 1e3:.1f} us, "
+    print(f"wgmma lm head n={n} k={k} m={m}: {ms.value * 1e3:.1f} us, "
           f"{n * k * 2 / (ms.value * 1e-3) / 1e9:.0f} GB/s")
 
 
 @pytest.mark.parametrize("name", ["gqa128_a0.1", "mha128_a0.1"])
 def test_engine_with_tcgen05_lm_head_stays_exact_and_within_the_margin_gate(name, monkeypatch):
-    """LSK_LMHEAD_TC=1: every LM head (draft, verify, autoregressive) goes through the tcgen05
+    """LSK_LMHEAD_TC=1: every LM head (draft, verify, autoregressive) goes through the wgmma
     kernel, so speculative == autoregressive must still hold exactly; against the oracle the usual
     margin gate applies (accumulation order differs from the mma.sync head)."""
     from layerskip_b200 import GenerationConfig

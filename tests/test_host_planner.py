@@ -9,7 +9,7 @@ from layerskip_b200.weights import ARCHS
 
 PRO_RMS, PRO_BF16 = 0, 1
 EPI_QKV, EPI_RESID, EPI_STORE, EPI_SILU, EPI_LMHEAD = range(5)
-SMS = 148
+SMS = 132                      # H100 SXM
 
 
 def plan(n_rows, k, m, pro, epi, sms=SMS):
@@ -47,9 +47,9 @@ def test_7b_schedules_match_design_md():
     p = plan(*g["qkv"][:2], 1, *g["qkv"][2:])
     assert (p.n_tiles, p.grid, p.n_chunks, p.ring_stages) == (768, 128, 1, 8)      # 768 = 6 x 128
     p = plan(*g["gate_up"][:2], 1, *g["gate_up"][2:])
-    assert (p.n_tiles, p.grid) == (1376, 138)                                      # 10 waves of 138
+    assert (p.n_tiles, p.grid) == (1376, 126)                                      # 11 waves of 126
     p = plan(*g["lm_head"][:2], 1, *g["lm_head"][2:])
-    assert (p.n_tiles, p.grid) == (2000, 143)
+    assert (p.n_tiles, p.grid) == (2000, 125)                                      # 16 waves of 125
     p1 = plan(*g["down"][:2], 1, *g["down"][2:])
     p7 = plan(*g["down"][:2], 7, *g["down"][2:])
     assert p1.n_chunks == 1 and p1.ring_stages == 8          # one resident row: no chunking
@@ -94,7 +94,7 @@ def test_attention_launch_plan_for_the_baseline_architectures():
     """engine.cu: attn_default_splits / plan_attention_launch (through lsk_plan_attention): the split
     count is min(4, SMs / local kv heads), the K/V ring is as deep as shared memory allows, and a grid
     that fits one wave gets more than half an SM's shared memory per CTA (one CTA per SM)."""
-    p = attn_plan(ARCHS["llama2-7b"], 7)                       # 32 kv heads: 32 x 4 CTAs on 148 SMs
+    p = attn_plan(ARCHS["llama2-7b"], 7)                       # 32 kv heads: 32 x 4 CTAs on 132 SMs
     assert (p.ok, p.n_splits, p.grid, p.ring_stages, p.row_blocks) == (1, 4, 128, 4, 1)
     assert p.smem_bytes > 114 * 1024 and p.kv_refetched_per_row_block == 1   # merge buffer aliases the ring
     p = attn_plan(ARCHS["llama3-8b"], 7)                       # GQA 4: 28 query rows -> 2 row blocks, K/V resident

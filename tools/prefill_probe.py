@@ -1,6 +1,6 @@
 """Prefill timing probe: python tools/prefill_probe.py [arch] [n_tokens ...]
 Device time of lsk_prefill (CUDA events on the engine's stream) for the given prompt lengths, with
-the tcgen05 path and (LSK_PREFILL_TC=0) the decode-kernel path."""
+the wgmma path and (LSK_PREFILL_TC=0) the decode-kernel path."""
 import os
 import sys
 
@@ -22,5 +22,5 @@ for n in lens:
         eng.begin(exit_layer=min(8, arch.layers), max_steps=8, eos_token_ids=[arch.vocab - 1])
         eng.prefill(ids)
         best = min(best, eng.last_device_ms)
-    print(f"prefill {n} tokens: {best:.3f} ms (tcgen05 path: {eng.prefill_tc})", flush=True)
+    print(f"prefill {n} tokens: {best:.3f} ms (wgmma path: {eng.prefill_tc})", flush=True)
 eng.close()

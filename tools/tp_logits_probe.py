@@ -1,6 +1,6 @@
 """torchrun --nproc-per-node N tools/tp_logits_probe.py arch [arch ...]
 max |logit(TP=N engine) - logit(single-GPU engine)| at the first decode step after a 128-id prompt,
-and after a 12-id prompt (decode-kernel prefill instead of the tcgen05 prefill)."""
+and after a 12-id prompt (decode-kernel prefill instead of the wgmma prefill)."""
 import os
 import sys
 
