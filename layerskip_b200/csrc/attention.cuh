@@ -1,6 +1,6 @@
 // attention.cuh — paged split-KV attention for decode / verify blocks (<= 16 query tokens).
 //
-// One CTA = (kv head, split); the splits of a kv head form a thread-block CLUSTER.  The query
+// One CTA = (kv head, split); no thread-block clusters (see the split merge below).  The query
 // rows of a CTA are all tokens x all q-heads that share the kv head (GQA), processed 16 rows at a
 // time as the M side of mma.sync m16n8k16.  A split owns the 64-key groups  s, s + n_splits, ...
 // (by ABSOLUTE key index, so the partition seen by a query at position p does not depend on how
@@ -17,20 +17,21 @@
 // fragments and the one boundary group (the keys this round appended) are still to be fetched.
 //
 // Partials (m, l, O) are merged in fixed order: the 4 warps of a CTA through shared memory, then
-// the splits through DISTRIBUTED shared memory after one cluster barrier.  Deterministic.
+// the splits: every split publishes its partial rows to global memory, and the LAST split of the kv
+// head to arrive (per-head arrival counter) merges all of them in split order.  Deterministic.  No
+// thread-block clusters: a cluster has to fit inside one GPC, and on the 132-SM H100 only 30
+// clusters of 4 (39 of 3) are resident at one CTA per SM, so a clustered 7B grid (32 x 4) or 13B
+// grid (40 x 3) would leave clusters for a second wave.  Unclustered, the grid is resident at once.
 #pragma once
-#include <cooperative_groups.h>
-
 #include "common.cuh"
 
 namespace lsk {
-namespace cg = cooperative_groups;
 
 constexpr int kAttnThreads = 128;
 constexpr int kKeyGroup = 64;                 // keys per pipeline stage (== one KV page)
 constexpr int kAttnMaxStages = 4;             // K/V stages in flight per CTA (AttnArgs::n_stages of them used)
-constexpr int kAttnHeader = 128;              // mbarriers
-constexpr int kMaxSplits = 8;                 // portable cluster size
+constexpr int kAttnHeader = 128;              // mbarriers, then the merger flag
+constexpr int kMaxSplits = 8;
 
 struct AttnArgs {
   const __nv_bfloat16* q;      // [M][q_ld] post-RoPE
@@ -53,7 +54,14 @@ struct AttnArgs {
   int reload_per_rb;           // 1: the merge buffer aliases the stages -> K/V re-fetched per row block
   int out_canon;               // 1: `out` is a canonical K-major operand (rows = tokens) for prefill_tc.cuh
   int n_stages;                // K/V ring depth (2 .. kAttnMaxStages)
+  float* part;                 // [n_kv_heads][n_splits][rows_pad][HD + 2] published partials (O, then m/l)
+  unsigned int* arrive;        // [n_kv_heads] splits done; zero between launches (the merger resets it)
 };
+
+// floats of AttnArgs::part for a launch
+__host__ inline size_t attn_part_floats(int n_kv_heads, int n_splits, int rows_pad, int hd) {
+  return (size_t)n_kv_heads * n_splits * rows_pad * (hd + 2);
+}
 
 // shared-memory plan of one launch (host and device agree through AttnArgs offsets)
 struct AttnSmemPlan {
@@ -81,10 +89,9 @@ __device__ __forceinline__ void team_sync() {
 }
 
 // Fixed-order merge of the splits' partials for one (row, 16-dim segment); `ml(s)` / `o(s)` return
-// split s's (m, l) pair and O segment (a peer CTA's shared memory).  SP = compile-time bound on
-// the number of splits: with SP <= 4 every remote value (4 (m, l) pairs + 16 float4) is requested
-// up front — ONE distributed-shared-memory round trip instead of a chain of five; same arithmetic
-// in the same order either way.
+// split s's (m, l) pair and O segment (published in global memory, read past L1).  SP = compile-time
+// bound on the number of splits: with SP <= 4 every value (4 (m, l) pairs + 16 float4) is requested
+// up front — ONE round trip instead of a chain of five; same arithmetic in the same order either way.
 template <int HD, int SP, typename FML, typename FO>
 __device__ __forceinline__ void merge_splits_write(const AttnArgs& a, int kvh, int row, int dseg,
                                                    FML ml, FO o) {
@@ -92,7 +99,7 @@ __device__ __forceinline__ void merge_splits_write(const AttnArgs& a, int kvh, i
 #pragma unroll
   for (int s = 0; s < SP; ++s) {
     ms[s] = -INFINITY; ls[s] = 0.f;
-    if (s < a.n_splits) { const float* p = ml(s); ms[s] = p[0]; ls[s] = p[1]; }
+    if (s < a.n_splits) { const float* p = ml(s); ms[s] = __ldcg(p); ls[s] = __ldcg(p + 1); }
   }
   float acc[16];
 #pragma unroll
@@ -104,7 +111,7 @@ __device__ __forceinline__ void merge_splits_write(const AttnArgs& a, int kvh, i
     for (int i = 0; i < 4; ++i)
 #pragma unroll
       for (int s = 0; s < SP; ++s)
-        v[i][s] = (s < a.n_splits) ? reinterpret_cast<const float4*>(o(s))[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[i][s] = (s < a.n_splits) ? __ldcg(reinterpret_cast<const float4*>(o(s)) + i) : make_float4(0.f, 0.f, 0.f, 0.f);
     float mm = -INFINITY;
 #pragma unroll
     for (int s = 0; s < SP; ++s) mm = fmaxf(mm, ms[s]);
@@ -139,7 +146,7 @@ __device__ __forceinline__ void merge_splits_write(const AttnArgs& a, int kvh, i
       float4 v[SP];
 #pragma unroll
       for (int s = 0; s < SP; ++s)
-        v[s] = (s < a.n_splits) ? reinterpret_cast<const float4*>(o(s))[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[s] = (s < a.n_splits) ? __ldcg(reinterpret_cast<const float4*>(o(s)) + i) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
       for (int s = 0; s < SP; ++s) {
         if (s < a.n_splits) {
@@ -172,14 +179,13 @@ __device__ __forceinline__ void merge_splits_write(const AttnArgs& a, int kvh, i
 
 template <int HD>
 __global__ void __launch_bounds__(kAttnThreads)
-attn_cluster_kernel(const AttnArgs a) {
+attn_split_kernel(const AttnArgs a) {
   constexpr int KS = HD / 16;                   // k steps of Q.K^T
   constexpr int DT = HD / 8;                    // n8 tiles of the output
   constexpr int CH = HD / 8;                    // 16-byte chunks per K/V row
   constexpr int kGroupBytes = kKeyGroup * HD * 2;
   constexpr int kStageBytes = 2 * kGroupBytes;  // K block, then V block
   extern __shared__ __align__(128) unsigned char dsm[];
-  cg::cluster_group cluster = cg::this_cluster();
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(dsm);
   uint64_t* empty_bar = full_bar + kAttnMaxStages;
   unsigned char* stages = dsm + kAttnHeader;
@@ -188,7 +194,8 @@ attn_cluster_kernel(const AttnArgs a) {
   float* mml = mo + 4 * 16 * HD;                                  // [4][16][2]
   float* po = reinterpret_cast<float*>(dsm + a.part_off);        // [rows_pad][HD]
   float* pml = po + (size_t)a.rows_pad * HD;                      // [rows_pad][2]
-  const int kvh = blockIdx.x, split = blockIdx.y;                 // cluster = all splits of one kv head
+  int* last = reinterpret_cast<int*>(empty_bar + kAttnMaxStages); // header word behind the mbarriers
+  const int kvh = blockIdx.x, split = blockIdx.y;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
 
@@ -406,17 +413,30 @@ attn_cluster_kernel(const AttnArgs a) {
     if (tid == 0 && rb + 1 < n_rb) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
 
-  // ---- merge the splits through distributed shared memory
-  cluster.sync();
+  // ---- publish this split's partial rows (same layout as po / pml)
+  const size_t part_floats = (size_t)a.rows_pad * (HD + 2);
+  float* gp = a.part + (size_t)(kvh * a.n_splits + split) * part_floats;
+  for (int i = tid; i < R * (HD / 4); i += kAttnThreads)
+    reinterpret_cast<float4*>(gp)[i] = reinterpret_cast<const float4*>(po)[i];
+  for (int i = tid; i < 2 * R; i += kAttnThreads) gp[(size_t)a.rows_pad * HD + i] = pml[i];
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) *last = atomicAdd(&a.arrive[kvh], 1u) == (unsigned)(a.n_splits - 1);
+  __syncthreads();
+  if (!*last) return;
+
+  // ---- the last split of the kv head merges every split's partial, in split order
+  __threadfence();
   constexpr int SEG = HD / 16;
-  for (int it = split * kAttnThreads + tid; it < R * SEG; it += a.n_splits * kAttnThreads) {
+  const float* hp = a.part + (size_t)kvh * a.n_splits * part_floats;
+  for (int it = tid; it < R * SEG; it += kAttnThreads) {
     const int row = it / SEG, dseg = (it % SEG) * 16;
-    auto f_ml = [&](int s) { return (const float*)cluster.map_shared_rank(pml, s) + row * 2; };
-    auto f_o = [&](int s) { return (const float*)cluster.map_shared_rank(po, s) + (size_t)row * HD + dseg; };
+    auto f_ml = [&](int s) { return hp + s * part_floats + (size_t)a.rows_pad * HD + row * 2; };
+    auto f_o = [&](int s) { return hp + s * part_floats + (size_t)row * HD + dseg; };
     if (a.n_splits <= 4) merge_splits_write<HD, 4>(a, kvh, row, dseg, f_ml, f_o);
     else merge_splits_write<HD, kMaxSplits>(a, kvh, row, dseg, f_ml, f_o);
   }
-  cluster.sync();      // nobody leaves while a peer may still read its partials
+  if (tid == 0) a.arrive[kvh] = 0u;   // every split has arrived: ready for the next launch
 }
 
 }  // namespace lsk

@@ -130,6 +130,9 @@ struct lsk_engine {
   float* hidden = nullptr;             // [16][hidden] fp32 residual-stream rows
   __nv_bfloat16* qbuf = nullptr;       // [16][q_rows]
   __nv_bfloat16* attn_out = nullptr;   // [16][q_rows]
+  float* attn_part = nullptr;          // attention: published split partials (AttnArgs::part)
+  size_t attn_part_cap = 0;            // floats
+  unsigned int* attn_arrive = nullptr; // attention: per-kv-head arrival counters (AttnArgs::arrive)
   __nv_bfloat16* act = nullptr;        // [16][inter_l]
   float* tp_buf = nullptr;             // [16][hidden] row-parallel partial sums (TP)
   float* logits = nullptr;             // [16][vocab_l_pad] (optional)
@@ -420,12 +423,12 @@ static AttnLaunchPlan plan_attention_launch(int head_dim, int group, int M, int 
   return p;
 }
 
-// Attention over the paged cache: the splits of one kv head = one thread-block cluster (DSMEM
-// merge); head_dim selects the instantiation, the shared-memory plan depends on (group, M).
+// Attention over the paged cache: grid (kv heads, splits), the last split of a head to finish
+// merges; head_dim selects the instantiation, the shared-memory plan depends on (group, M).
 template <int HD>
 static int launch_attention_t(lsk_engine* e, AttnArgs& a) {
   static std::atomic<uint64_t> configured{0};
-  auto kern = attn_cluster_kernel<HD>;
+  auto kern = attn_split_kernel<HD>;
   int dev = 0;
   CU(cudaGetDevice(&dev));
   const uint64_t bit = 1ull << (dev & 63);
@@ -440,6 +443,9 @@ static int launch_attention_t(lsk_engine* e, AttnArgs& a) {
     return fail(LSK_ERR_INVALID, "attention: %d query rows per kv head do not fit shared memory", a.group * a.M);
   a.rows_pad = (a.group * a.M + 15) / 16 * 16;
   a.merge_off = sp.merge_off; a.part_off = sp.part_off; a.reload_per_rb = sp.reload_per_rb;
+  if (attn_part_floats(a.n_kv_heads, a.n_splits, a.rows_pad, HD) > e->attn_part_cap)
+    return fail(LSK_ERR_INVALID, "attention: %d query rows per kv head exceed the partials buffer", a.group * a.M);
+  a.part = e->attn_part; a.arrive = e->attn_arrive;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(a.n_kv_heads, a.n_splits);
   cfg.blockDim = dim3(kAttnThreads);
@@ -447,13 +453,11 @@ static int launch_attention_t(lsk_engine* e, AttnArgs& a) {
   // CTAs then spread over the SMs instead of sharing a few SMs' load bandwidth
   cfg.dynamicSmemBytes = lp.smem;
   cfg.stream = e->stream;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = a.n_splits; at[0].val.clusterDim.z = 1;
-  at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[1].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  cfg.numAttrs = e->use_pdl ? 2 : 1;
+  cfg.numAttrs = e->use_pdl ? 1 : 0;
   e->launches += 1;
   e->capture_launches += 1;
   if (!e->profiling) {
@@ -476,6 +480,16 @@ static int launch_attention(lsk_engine* e, AttnArgs& a, int head_dim) {
     case 32: return launch_attention_t<32>(e, a);
     default: return fail(LSK_ERR_INVALID, "head_dim %d unsupported (32, 64 or 128)", head_dim);
   }
+}
+
+// Split partials + arrival counters of the attention kernel, sized for `rows` query tokens per
+// launch (the prompt pass's 128) at the engine's split count; the counters start at zero.
+static int alloc_attn_partials(lsk_engine* e, int kv_heads, int group, int head_dim, int rows) {
+  e->attn_part_cap = attn_part_floats(kv_heads, e->n_splits, (group * rows + 15) / 16 * 16, head_dim);
+  CU(cudaMalloc((void**)&e->attn_part, e->attn_part_cap * 4));
+  CU(cudaMalloc((void**)&e->attn_arrive, (size_t)kv_heads * 4));
+  CU(cudaMemsetAsync(e->attn_arrive, 0, (size_t)kv_heads * 4, e->stream));
+  return LSK_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -978,7 +992,7 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
   // split-KV factor: a constant of the engine (results are batch-invariant only for a fixed
   // partition).  The kernel is bound by per-SM load bandwidth and barrier latency, so the grid is
   // ONE CTA per SM on as many SMs as possible — splits = floor(SMs / kv heads), at most 4 (7B: 32
-  // heads x 4 splits; an 8-CTA cluster's barrier and 8-way merge cost more than extra SMs bring).
+  // heads x 4 splits; an 8-way split's merge costs more than extra SMs bring).
   e->n_splits = c.attn_splits > 0 ? c.attn_splits : attn_default_splits(e->sm_count, e->kv_heads_l);
   if (const char* env = getenv("LSK_ATTN_SPLITS")) e->n_splits = atoi(env);   // clamped to [1, 8] below
   if (const char* env = getenv("LSK_ATTN_STAGES")) e->attn_stages = atoi(env);
@@ -1076,6 +1090,7 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
   TRY(alloc((void**)&e->hidden, (size_t)(kMaxRows + 1) * h * 4));
   TRY(alloc((void**)&e->qbuf, (size_t)kMaxRows * e->q_rows * 2));
   TRY(alloc((void**)&e->attn_out, (size_t)kMaxRows * e->q_rows * 2));
+  TRY(alloc_attn_partials(e, e->kv_heads_l, e->group, c.head_dim, std::max(kMaxRows, 128)));
   TRY(alloc((void**)&e->act, (size_t)kMaxRows * e->inter_l_pad * 2));   // pad columns stay zero
   TRY(alloc((void**)&e->tp_buf, (size_t)kMaxRows * h * 4));
   if (e->keep_logits) TRY(alloc((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4));
@@ -1149,7 +1164,7 @@ void lsk_destroy(lsk_engine* e) {
   void* ptrs[] = {e->embed, e->final_norm, e->lm_head, e->lm_head_tc, e->kpool, e->vpool, e->page_table, e->rope,
                   e->hidden, e->qbuf, e->attn_out, e->act, e->tp_buf, e->logits, e->logits_gath, e->logits_full, e->probs_d, e->probs_v, e->samp_scratch, e->cand_val,
                   e->cand_idx, e->gath_val, e->gath_idx, e->ban_val, e->ban_idx, e->rank_val, e->rank_idx,
-                  e->d_zero, e->d_prompt, e->state, e->gen_dev};
+                  e->d_zero, e->d_prompt, e->state, e->gen_dev, e->attn_part, e->attn_arrive};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->res_host) cudaFreeHost(e->res_host);
   if (e->ev0) cudaEventDestroy(e->ev0);
@@ -1775,7 +1790,7 @@ __global__ void paginate_kv_kernel(const __nv_bfloat16* __restrict__ src, int n_
 // Stand-alone attention (unit test / micro-benchmark): m query rows at positions ctx-m .. ctx-1
 // attend causally to keys 0 .. ctx-1.  q / out: [m][n_heads * 128] bf16; k / v: natural
 // [n_kv_heads][ctx][128] bf16 (k already rotated); page_perm (host, may be null) permutes the
-// logical -> physical page map.  Same launch path as the engine (cluster kernel).
+// logical -> physical page map.  Same launch path as the engine.
 int lsk_test_attn(const void* q, const void* k, const void* v, int32_t n_heads, int32_t n_kv_heads,
                   int32_t head_dim, int32_t ctx, int32_t m, int32_t n_splits, const int32_t* page_perm, void* out,
                   int32_t iters, float* avg_ms) {
@@ -1792,6 +1807,8 @@ int lsk_test_attn(const void* q, const void* k, const void* v, int32_t n_heads, 
   }
   CU(cudaStreamCreateWithFlags(&tmp.stream, cudaStreamNonBlocking));
   tmp.use_pdl = true;
+  tmp.n_splits = n_splits;
+  TRY(alloc_attn_partials(&tmp, n_kv_heads, n_heads / n_kv_heads, head_dim, m));
   const int n_pages = (ctx + kPageTokens - 1) / kPageTokens;
   const size_t pool_elems = (size_t)n_pages * n_kv_heads * kPageTokens * kHeadDim;
   __nv_bfloat16 *kp = nullptr, *vp = nullptr;
@@ -1838,7 +1855,7 @@ int lsk_test_attn(const void* q, const void* k, const void* v, int32_t n_heads, 
     CU(cudaEventDestroy(e0));
     CU(cudaEventDestroy(e1));
   }
-  cudaFree(kp); cudaFree(vp); cudaFree(pt); cudaFree(len);
+  cudaFree(kp); cudaFree(vp); cudaFree(pt); cudaFree(len); cudaFree(tmp.attn_part); cudaFree(tmp.attn_arrive);
   CU(cudaStreamDestroy(tmp.stream));
   tmp.stream = nullptr;
   return LSK_OK;

@@ -51,6 +51,9 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
         + MAX_ROWS * h * 4                     # TP partial sums
         + max_pos * (arch.head_dim // 2) * 8 + max_pos * 4 + n_pages * 4   # RoPE table, prompt ids, page table
         + SM_COUNT * MAX_ROWS * 8 + tp_size * MAX_ROWS * 8)      # arg-max candidates
+    kvh_l = arch.kv_heads // tp_size                          # attention split partials + counters
+    splits = max(1, min(4, SM_COUNT // kvh_l))
+    scratch += kvh_l * splits * ((arch.heads // arch.kv_heads * 128 + 15) // 16 * 16) * (arch.head_dim + 2) * 4 + kvh_l * 4
     if prefill_tc and h % 64 == 0:
         scratch += 6 * 128 * h * 4 + 128 * q_l * 2 + 16384 * (h // 64 + (q_l + 63) // 64 + (inter_l + 63) // 64)
     if keep_logits or sampling:
