@@ -164,11 +164,12 @@ int lsk_debug_forward_rows(lsk_engine* e, const int32_t* ids_host, int32_t m);
 typedef enum {
   LSK_DBG_HIDDEN = 0,        /* fp32 [16, hidden] residual-stream rows of the last launch     */
   LSK_DBG_LOGITS = 1,        /* fp32 [16, vocab_local] (needs LSK_FLAG_KEEP_LOGITS)           */
-  LSK_DBG_KROW = 2,          /* bf16->fp32 K cache row [head_dim]: layer, index = kv_head*max_ctx + pos */
+  LSK_DBG_KROW = 2,          /* bf16->fp32 K cache rows [count][head_dim], n_floats = count*head_dim: layer, index = kv_head*max_ctx + pos0; positions pos0 .. pos0+count-1 (<= max_ctx) */
   LSK_DBG_VROW = 3,
   LSK_DBG_PROBS_DRAFT = 4,   /* fp32 [16, vocab] warped (T, top-k, top-p) draft distributions     */
   LSK_DBG_PROBS_VERIFY = 5,  /* fp32 [16, vocab] warped verifier distributions of the last round */
-  LSK_DBG_RESIDUAL = 6       /* fp32 [vocab] max(p_verify - p_draft, 0) of the last rejected draft (unnormalised; self_speculation_generator.py:27-29 max_fn before its division) */
+  LSK_DBG_RESIDUAL = 6,      /* fp32 [vocab] max(p_verify - p_draft, 0) of the last rejected draft (unnormalised; self_speculation_generator.py:27-29 max_fn before its division) */
+  LSK_DBG_ARGMAX = 7         /* fp32 [rows][2] (logit, token id) the engine picks greedily per row of the last LM head, n_floats = 2*rows (<= 32): its candidates merged as the accept kernels merge them */
 } lsk_debug_what;
 int lsk_debug_read(lsk_engine* e, int32_t what, int32_t layer, int64_t index,
                    float* dst_host, int64_t n_floats);
@@ -226,7 +227,9 @@ int lsk_test_gemm(const void* packed_dev, int64_t n, int64_t k, const void* x_bf
  * 0 .. ctx-1 (modeling_llama.py:187-221 eager attention).  q / out: [m][n_heads*head_dim] bf16,
  * k / v: natural [n_kv_heads][ctx][head_dim] bf16 (k already rotated) — the entry point builds the
  * engine's paged, swizzled pool from them; page_perm_host (nullable) permutes logical->physical
- * pages.  All other pointers are device pointers. */
+ * pages.  m <= 16 runs one decode block; 16 < m <= 128 runs the prompt pass's launches for one
+ * chunk at position ctx-m (canonical output, returned unpacked in the same [m][n_heads*head_dim]
+ * layout).  All other pointers are device pointers. */
 int lsk_test_attn(const void* q_dev, const void* k_dev, const void* v_dev, int32_t n_heads,
                   int32_t n_kv_heads, int32_t head_dim, int32_t ctx, int32_t m, int32_t n_splits,
                   const int32_t* page_perm_host, void* out_dev, int32_t iters, float* avg_ms_out);

@@ -24,7 +24,7 @@ LSK_ROPE_DEFAULT, LSK_ROPE_LINEAR, LSK_ROPE_LLAMA3 = 0, 1, 2
  LSK_W_LN2, LSK_W_GATE, LSK_W_UP, LSK_W_DOWN) = range(12)
 
 LSK_DBG_HIDDEN, LSK_DBG_LOGITS, LSK_DBG_KROW, LSK_DBG_VROW, LSK_DBG_PROBS_DRAFT, \
-    LSK_DBG_PROBS_VERIFY, LSK_DBG_RESIDUAL = range(7)
+    LSK_DBG_PROBS_VERIFY, LSK_DBG_RESIDUAL, LSK_DBG_ARGMAX = range(8)
 
 
 class LskLibraryError(RuntimeError):

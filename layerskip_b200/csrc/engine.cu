@@ -158,7 +158,7 @@ struct lsk_engine {
 
   GemmPlan p_qkv, p_o, p_gu, p_d, p_lm;
   size_t l2_prefetch_bytes = 0;          // LSK_L2_PREFETCH_MB: head of the NEXT kernel's weights pulled into L2 (A/B: no gain, +11 % traffic -> off)
-  int lm_cand = 0;                     // candidates produced by the LM head (its grid)
+  int lm_cand = 0;                     // candidates produced by the wgmma LM head (its grid)
   const float* cur_cand_val = nullptr;  // candidates of the last enqueued LM head (epilogue's, or the banned rows' arg-max)
   const int* cur_cand_idx = nullptr;
   int cur_n_cand = 0;
@@ -592,16 +592,38 @@ static int launch_prefill_gemm(lsk_engine* e, PrefillGemmArgs& a) {
   return LSK_OK;
 }
 
+// Prompt-pass attention of m <= 128 token rows at positions c0 .. c0+m-1 (q: [m][q_ld]) over the keys
+// 0 .. c0+m-1 of the paged cache.  The base length is the device zero `zero`, the positions come from
+// pos_off, and the output goes to the canonical operand `out_canon` (rows = token index in the chunk)
+// that the O projection of prefill_tc.cuh reads.  One launch per m_attn rows: as many as fit the
+// attention kernel's shared-memory plan (a multiple of 16, so the canonical swizzle of row r0 + j
+// equals that of row j).
+static int launch_prompt_attention(lsk_engine* e, const __nv_bfloat16* q, int q_ld, unsigned char* out_canon,
+                                   const __nv_bfloat16* kp, const __nv_bfloat16* vp, const int* page_table,
+                                   const int* zero, int c0, int m, int group, int n_kv_heads, int head_dim) {
+  int m_attn = 16;
+  for (int cand = kPfTokens; cand >= 16; cand -= 16)
+    if (attn_smem_plan(head_dim, group, cand, 2).total <= (size_t)kSmemMax) { m_attn = cand; break; }
+  for (int r0 = 0; r0 < m; r0 += m_attn) {
+    AttnArgs a{};
+    a.q = q + (size_t)r0 * q_ld; a.q_ld = q_ld;
+    // operand rows are addressed by token index inside the 128-row stage: shift by r0 rows
+    a.out = reinterpret_cast<__nv_bfloat16*>(out_canon + canon_offset(r0, 0)); a.out_canon = 1;
+    a.kpool = kp; a.vpool = vp; a.page_table = page_table;
+    a.base_len = zero; a.pos_off = c0 + r0; a.M = (m - r0) < m_attn ? (m - r0) : m_attn;
+    a.group = group; a.n_kv_heads = n_kv_heads; a.n_splits = e->n_splits;
+    a.scale = 1.0f / sqrtf((float)head_dim);
+    TRY(launch_attention(e, a, head_dim));
+  }
+  return LSK_OK;
+}
+
 static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m) {
   const lsk_config& c = e->cfg;
   const bool tp = c.tp_size > 1;
   e->cur_class = CLS_MISC;
   CU(launch(e, embed_tokens_kernel, dim3(m), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
             (const int*)(e->d_prompt + c0), e->hidden_p, c.hidden));
-  // rows of one attention launch: as many as fit its shared-memory plan (multiple of 16)
-  int m_attn = 16;
-  for (int cand = kPfTokens; cand >= 16; cand -= 16)
-    if (attn_smem_plan(c.head_dim, e->group, cand, 2).total <= (size_t)kSmemMax) { m_attn = cand; break; }
   // row-parallel GEMMs (O / down): hidden / 128 feature tiles are too few to keep the SMs streaming
   // -> split K; the partial tiles are summed (fixed order) by the next rms_canon_kernel
   const int ks_o = std::max(1, std::min(std::min(4, e->kst_q), e->sm_count / e->pf_t_h));
@@ -641,17 +663,8 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m) {
     // K/V rows are written nothing downstream is needed
     if (li + 1 == c.n_layers) break;
     e->cur_class = CLS_ATTN;
-    for (int r0 = 0; r0 < m; r0 += m_attn) {
-      AttnArgs a{};
-      a.q = e->q_p + (size_t)r0 * e->q_rows; a.q_ld = e->q_rows;
-      // operand rows are addressed by token index inside the 128-row stage: shift by r0 rows
-      a.out = reinterpret_cast<__nv_bfloat16*>(e->attn_c + canon_offset(r0, 0)); a.out_canon = 1;
-      a.kpool = kp; a.vpool = vp; a.page_table = e->page_table;
-      a.base_len = e->d_zero; a.pos_off = c0 + r0; a.M = (m - r0) < m_attn ? (m - r0) : m_attn;
-      a.group = e->group; a.n_kv_heads = e->kv_heads_l; a.n_splits = e->n_splits;
-      a.scale = 1.0f / sqrtf((float)c.head_dim);
-      TRY(launch_attention(e, a, c.head_dim));
-    }
+    TRY(launch_prompt_attention(e, e->q_p, e->q_rows, e->attn_c, kp, vp, e->page_table, e->d_zero, c0, m,
+                                e->group, e->kv_heads_l, c.head_dim));
     e->cur_class = CLS_O;
     {
       PrefillGemmArgs a{};
@@ -754,7 +767,10 @@ static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0, const void* a
   e->cur_class = CLS_MISC;
   const float* cv = e->cand_val;
   const int* ci = e->cand_idx;
-  int ncand = e->lm_cand;
+  // one candidate per CTA of the launch: the skinny GEMM's grid depends on M (plan_sched, exactly as
+  // launch_gemm picks it) and may be smaller than min(tiles, SMs) — candidates past it are never
+  // written and must not be merged (a stale (0, 0) would beat a row whose logits are all negative)
+  int ncand = e->lm_tc ? e->lm_cand : plan_sched(M <= 8 ? 1 : 2, M, PRO_RMS, EPI_LMHEAD, e->p_lm, e->sm_count).grid;
   if (ban) {
     CU(launch(e, ngram_ban_kernel, dim3(M), dim3(256), 0, e->logits, e->vocab_l_pad, e->vocab_l, e->vocab_off,
               (const int*)e->d_prompt, (const DevState*)e->state, (int)e->gen.no_repeat_ngram_size, j0));
@@ -1006,7 +1022,6 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
   e->p_gu = make_plan(2 * e->inter_l, c.hidden, e->sm_count);
   e->p_d = make_plan(c.hidden, e->inter_l_pad, e->sm_count);
   e->p_lm = make_plan(e->vocab_l_pad, c.hidden, e->sm_count);
-  e->lm_cand = e->p_lm.n_tiles < e->sm_count ? e->p_lm.n_tiles : e->sm_count;
   if (const char* env = getenv("LSK_L2_PREFETCH_MB")) e->l2_prefetch_bytes = (size_t)atoi(env) << 20;
   if (getenv("LSK_LMHEAD_TC") && atoi(getenv("LSK_LMHEAD_TC")) != 0) {
     // wgmma LM head: needs hidden % 64 == 0 and the 16-token B operand + a >= 3-stage ring in
@@ -1624,21 +1639,51 @@ int lsk_debug_read(lsk_engine* e, int32_t what, int32_t layer, int64_t index, fl
     CU(cudaMemcpy(dst, e->logits, (size_t)n * 4, cudaMemcpyDeviceToHost));
     return LSK_OK;
   }
+  if (what == LSK_DBG_ARGMAX) {
+    // the engine's greedy choice per row of the last LM head: its candidates merged by the same
+    // fixed-order reduction as the accept kernels (reduce_candidates / rank_best_kernel)
+    if (!e->cur_cand_val || !e->cur_cand_idx) return fail(LSK_ERR_STATE, "no LM head has run");
+    if (n < 2 || n % 2 || n > 2 * kMaxRows) return fail(LSK_ERR_INVALID, "n = 2 * rows (value, index), rows <= %d", kMaxRows);
+    const int rows = (int)(n / 2);
+    rank_best_kernel<<<1, 32 * kMaxRows, 0, e->stream>>>(cand_val_ptr(e), cand_idx_ptr(e), n_cand(e), rows,
+                                                          e->rank_val, e->rank_idx);
+    CU(cudaGetLastError());
+    float val[kMaxRows];
+    int idx[kMaxRows];
+    CU(cudaMemcpyAsync(val, e->rank_val, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaMemcpyAsync(idx, e->rank_idx, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    for (int r = 0; r < rows; ++r) { dst[2 * r] = val[r]; dst[2 * r + 1] = (float)idx[r]; }
+    return LSK_OK;
+  }
   if (what == LSK_DBG_KROW || what == LSK_DBG_VROW) {
+    // n = count * head_dim: `count` consecutive positions of one kv head, pos0 .. pos0 + count - 1
     const int hd = e->cfg.head_dim;
-    if (layer < 0 || layer >= e->cfg.n_layers || n != hd) return fail(LSK_ERR_INVALID, "bad layer / n (one row = head_dim floats)");
-    const int64_t head = index / e->cfg.max_ctx, pos = index % e->cfg.max_ctx;
+    if (layer < 0 || layer >= e->cfg.n_layers || n < hd || n % hd)
+      return fail(LSK_ERR_INVALID, "bad layer / n (a multiple of head_dim floats: one row per position)");
+    const int64_t head = index / e->cfg.max_ctx, pos0 = index % e->cfg.max_ctx, count = n / hd;
     if (head >= e->kv_heads_l) return fail(LSK_ERR_INVALID, "bad kv head");
+    if (pos0 + count > e->cfg.max_ctx) return fail(LSK_ERR_INVALID, "rows %lld .. %lld cross max_ctx", (long long)pos0,
+                                                   (long long)(pos0 + count - 1));
     std::vector<int> pt(e->n_pages);
     CU(cudaMemcpy(pt.data(), e->page_table, pt.size() * 4, cudaMemcpyDeviceToHost));
     const __nv_bfloat16* pool = (what == LSK_DBG_KROW ? e->kpool : e->vpool) + (size_t)layer * e->pool_layer_elems;
-    // one token row is contiguous; its 16-byte chunks are swizzled (common.cuh: kv_elem_offset)
-    const __nv_bfloat16* src = pool + kv_elem_offset(hd, pt[pos >> 6], e->kv_heads_l, (int)head, (int)(pos & 63), 0) -
-                               (size_t)(kv_chunk_swizzle(hd, (int)(pos & 63)) * 8);
-    std::vector<__nv_bfloat16> tmp(hd);
-    CU(cudaMemcpy(tmp.data(), src, (size_t)hd * 2, cudaMemcpyDeviceToHost));
-    for (int i = 0; i < hd; ++i)
-      dst[i] = __bfloat162float(tmp[(((i >> 3) ^ kv_chunk_swizzle(hd, (int)(pos & 63))) << 3) + (i & 7)]);
+    // the token rows of one (page, kv head) block are contiguous; inside a row the 16-byte chunks
+    // are swizzled (common.cuh: kv_elem_offset): one copy per page, then unswizzle row by row
+    std::vector<__nv_bfloat16> tmp((size_t)kPageTokens * hd);
+    for (int64_t p = pos0; p < pos0 + count;) {
+      const int tok0 = (int)(p & 63);
+      const int rows = (int)std::min<int64_t>(kPageTokens - tok0, pos0 + count - p);
+      const __nv_bfloat16* src = pool + kv_elem_offset(hd, pt[p >> 6], e->kv_heads_l, (int)head, tok0, 0) -
+                                 (size_t)(kv_chunk_swizzle(hd, tok0) * 8);
+      CU(cudaMemcpy(tmp.data(), src, (size_t)rows * hd * 2, cudaMemcpyDeviceToHost));
+      for (int r = 0; r < rows; ++r) {
+        const int swz = kv_chunk_swizzle(hd, tok0 + r);
+        float* d = dst + (size_t)(p - pos0 + r) * hd;
+        for (int i = 0; i < hd; ++i) d[i] = __bfloat162float(tmp[(size_t)r * hd + (((i >> 3) ^ swz) << 3) + (i & 7)]);
+      }
+      p += rows;
+    }
     return LSK_OK;
   }
   return fail(LSK_ERR_INVALID, "unknown debug selector %d", what);
@@ -1787,19 +1832,49 @@ __global__ void paginate_kv_kernel(const __nv_bfloat16* __restrict__ src, int n_
   }
 }
 
+// canonical operand rows [m][cols] (common.cuh: canon_offset) -> natural bf16 [m][cols]
+__global__ void uncanon_rows_kernel(const unsigned char* __restrict__ src, int m, int cols,
+                                    __nv_bfloat16* __restrict__ dst) {
+  const int chunks = cols >> 3;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m * chunks; i += gridDim.x * blockDim.x) {
+    const int row = i / chunks, k = (i % chunks) * 8;
+    *reinterpret_cast<uint4*>(dst + (size_t)row * cols + k) = *reinterpret_cast<const uint4*>(src + canon_offset(row, k));
+  }
+}
+
 // Stand-alone attention (unit test / micro-benchmark): m query rows at positions ctx-m .. ctx-1
-// attend causally to keys 0 .. ctx-1.  q / out: [m][n_heads * 128] bf16; k / v: natural
-// [n_kv_heads][ctx][128] bf16 (k already rotated); page_perm (host, may be null) permutes the
-// logical -> physical page map.  Same launch path as the engine.
+// attend causally to keys 0 .. ctx-1.  q / out: [m][n_heads * head_dim] bf16; k / v: natural
+// [n_kv_heads][ctx][head_dim] bf16 (k already rotated); page_perm (host, may be null) permutes the
+// logical -> physical page map.  Same launch paths as the engine: m <= 16 rows are one decode block
+// (base length ctx - m); 16 < m <= 128 rows are one prompt-pass chunk at c0 = ctx - m
+// (launch_prompt_attention: base length 0, canonical output, unpacked here to [m][n_heads * head_dim]).
 int lsk_test_attn(const void* q, const void* k, const void* v, int32_t n_heads, int32_t n_kv_heads,
                   int32_t head_dim, int32_t ctx, int32_t m, int32_t n_splits, const int32_t* page_perm, void* out,
                   int32_t iters, float* avg_ms) {
   const int kHeadDim = head_dim;
   if (head_dim != 32 && head_dim != 64 && head_dim != 128) return fail(LSK_ERR_INVALID, "head_dim %d unsupported", head_dim);
   if (!q || !k || !v || !out || n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads || ctx < m || m < 1 ||
-      m > kMaxRows || n_splits < 1 || n_splits > 8)
+      m > kPfTokens || n_splits < 1 || n_splits > 8)
     return fail(LSK_ERR_INVALID, "bad attention test shape");
+  const bool prompt = m > kMaxRows;
   lsk_engine tmp;
+  // every buffer, event and the stream are released on every return path (errors included)
+  struct Owned {
+    lsk_engine& t;
+    __nv_bfloat16 *kp = nullptr, *vp = nullptr;
+    int *pt = nullptr, *len = nullptr;
+    unsigned char* canon = nullptr;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    ~Owned() {
+      if (t.stream) cudaStreamSynchronize(t.stream);
+      void* bufs[] = {kp, vp, pt, len, canon, t.attn_part, t.attn_arrive};
+      for (void* b : bufs) if (b) cudaFree(b);
+      if (e0) cudaEventDestroy(e0);
+      if (e1) cudaEventDestroy(e1);
+      if (t.stream) cudaStreamDestroy(t.stream);
+      t.stream = nullptr;
+    }
+  } o{tmp};
   {
     int dev = 0;
     CU(cudaGetDevice(&dev));
@@ -1811,53 +1886,55 @@ int lsk_test_attn(const void* q, const void* k, const void* v, int32_t n_heads, 
   TRY(alloc_attn_partials(&tmp, n_kv_heads, n_heads / n_kv_heads, head_dim, m));
   const int n_pages = (ctx + kPageTokens - 1) / kPageTokens;
   const size_t pool_elems = (size_t)n_pages * n_kv_heads * kPageTokens * kHeadDim;
-  __nv_bfloat16 *kp = nullptr, *vp = nullptr;
-  int *pt = nullptr, *len = nullptr;
-  CU(cudaMalloc((void**)&kp, pool_elems * 2));
-  CU(cudaMalloc((void**)&vp, pool_elems * 2));
-  CU(cudaMalloc((void**)&pt, (size_t)n_pages * 4));
-  CU(cudaMalloc((void**)&len, 4));
-  CU(cudaMemsetAsync(kp, 0, pool_elems * 2, tmp.stream));
-  CU(cudaMemsetAsync(vp, 0, pool_elems * 2, tmp.stream));
   std::vector<int> pth(n_pages);
   for (int i = 0; i < n_pages; ++i) pth[i] = page_perm ? page_perm[i] : i;
   for (int i = 0; i < n_pages; ++i)
     if (pth[i] < 0 || pth[i] >= n_pages) return fail(LSK_ERR_INVALID, "bad page permutation");
-  const int base = ctx - m;
-  CU(cudaMemcpyAsync(pt, pth.data(), (size_t)n_pages * 4, cudaMemcpyHostToDevice, tmp.stream));
-  CU(cudaMemcpyAsync(len, &base, 4, cudaMemcpyHostToDevice, tmp.stream));
-  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)k, n_kv_heads, ctx, head_dim, pt, kp);
-  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)v, n_kv_heads, ctx, head_dim, pt, vp);
+  CU(cudaMalloc((void**)&o.kp, pool_elems * 2));
+  CU(cudaMalloc((void**)&o.vp, pool_elems * 2));
+  CU(cudaMalloc((void**)&o.pt, (size_t)n_pages * 4));
+  CU(cudaMalloc((void**)&o.len, 4));
+  CU(cudaMemsetAsync(o.kp, 0, pool_elems * 2, tmp.stream));
+  CU(cudaMemsetAsync(o.vp, 0, pool_elems * 2, tmp.stream));
+  const int base = prompt ? 0 : ctx - m;
+  const int q_cols = n_heads * kHeadDim;
+  if (prompt) {
+    CU(cudaMalloc((void**)&o.canon, (size_t)((q_cols + 63) / 64) * kCanonStageBytes));
+    CU(cudaMemsetAsync(o.canon, 0, (size_t)((q_cols + 63) / 64) * kCanonStageBytes, tmp.stream));
+  }
+  CU(cudaMemcpyAsync(o.pt, pth.data(), (size_t)n_pages * 4, cudaMemcpyHostToDevice, tmp.stream));
+  CU(cudaMemcpyAsync(o.len, &base, 4, cudaMemcpyHostToDevice, tmp.stream));
+  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)k, n_kv_heads, ctx, head_dim, o.pt, o.kp);
+  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)v, n_kv_heads, ctx, head_dim, o.pt, o.vp);
   CU(cudaGetLastError());
   AttnArgs a{};
-  a.q = (const __nv_bfloat16*)q; a.q_ld = n_heads * kHeadDim;
-  a.out = (__nv_bfloat16*)out; a.out_ld = n_heads * kHeadDim;
-  a.kpool = kp; a.vpool = vp; a.page_table = pt; a.base_len = len; a.pos_off = 0; a.M = m;
+  a.q = (const __nv_bfloat16*)q; a.q_ld = q_cols;
+  a.out = (__nv_bfloat16*)out; a.out_ld = q_cols;
+  a.kpool = o.kp; a.vpool = o.vp; a.page_table = o.pt; a.base_len = o.len; a.pos_off = 0; a.M = m;
   a.group = n_heads / n_kv_heads; a.n_kv_heads = n_kv_heads; a.n_splits = n_splits;
   a.scale = 1.0f / sqrtf((float)kHeadDim);
-  int st = launch_attention(&tmp, a, head_dim);
-  if (st != LSK_OK) return st;
+  auto run = [&]() -> int {
+    if (!prompt) return launch_attention(&tmp, a, head_dim);
+    return launch_prompt_attention(&tmp, (const __nv_bfloat16*)q, q_cols, o.canon, o.kp, o.vp, o.pt, o.len, ctx - m, m,
+                                   n_heads / n_kv_heads, n_kv_heads, head_dim);
+  };
+  TRY(run());
+  if (prompt) {
+    uncanon_rows_kernel<<<tmp.sm_count, 256, 0, tmp.stream>>>(o.canon, m, q_cols, (__nv_bfloat16*)out);
+    CU(cudaGetLastError());
+  }
   CU(cudaStreamSynchronize(tmp.stream));
   if (iters > 0) {
-    cudaEvent_t e0, e1;
-    CU(cudaEventCreate(&e0));
-    CU(cudaEventCreate(&e1));
-    CU(cudaEventRecord(e0, tmp.stream));
-    for (int i = 0; i < iters; ++i) {
-      st = launch_attention(&tmp, a, head_dim);
-      if (st != LSK_OK) return st;
-    }
-    CU(cudaEventRecord(e1, tmp.stream));
-    CU(cudaEventSynchronize(e1));
+    CU(cudaEventCreate(&o.e0));
+    CU(cudaEventCreate(&o.e1));
+    CU(cudaEventRecord(o.e0, tmp.stream));
+    for (int i = 0; i < iters; ++i) TRY(run());
+    CU(cudaEventRecord(o.e1, tmp.stream));
+    CU(cudaEventSynchronize(o.e1));
     float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, e0, e1));
+    CU(cudaEventElapsedTime(&ms, o.e0, o.e1));
     if (avg_ms) *avg_ms = ms / iters;
-    CU(cudaEventDestroy(e0));
-    CU(cudaEventDestroy(e1));
   }
-  cudaFree(kp); cudaFree(vp); cudaFree(pt); cudaFree(len); cudaFree(tmp.attn_part); cudaFree(tmp.attn_arrive);
-  CU(cudaStreamDestroy(tmp.stream));
-  tmp.stream = nullptr;
   return LSK_OK;
 }
 

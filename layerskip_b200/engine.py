@@ -244,6 +244,15 @@ class Engine:
             _lib.check(self._lib.lsk_debug_forward_rows(self._h, arr, m))
         return self.debug_logits(m)
 
+    def debug_argmax(self, rows: int):
+        """The engine's greedy choice for each of the first `rows` rows of the last LM head (the
+        LM-head epilogue's candidates merged as the accept kernels merge them): (logits, token ids)."""
+        buf = (C.c_float * (2 * rows))()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_debug_read(self._h, _lib.LSK_DBG_ARGMAX, 0, 0, buf, 2 * rows))
+        t = torch.frombuffer(buf, dtype=torch.float32).clone().view(rows, 2)
+        return t[:, 0], t[:, 1].to(torch.int64)
+
     def debug_hidden(self, rows: int = 16) -> torch.Tensor:
         n = rows * self.arch.hidden
         buf = (C.c_float * n)()
@@ -278,13 +287,18 @@ class Engine:
         return torch.frombuffer(buf, dtype=torch.float32).clone()
 
     def debug_kv_row(self, which: str, layer: int, kv_head: int, pos: int) -> torch.Tensor:
+        return self.debug_kv_rows(which, layer, kv_head, pos, 1)[0]
+
+    def debug_kv_rows(self, which: str, layer: int, kv_head: int, pos0: int, count: int) -> torch.Tensor:
+        """K ('k') or V ('v') cache rows of one kv head at positions pos0 .. pos0+count-1 as fp32
+        [count, head_dim] (bf16 values), in one call."""
         hd = self.arch.head_dim
-        buf = (C.c_float * hd)()
+        buf = (C.c_float * (count * hd))()
         what = _lib.LSK_DBG_KROW if which == "k" else _lib.LSK_DBG_VROW
         with torch.cuda.device(self.device):
-            _lib.check(self._lib.lsk_debug_read(self._h, what, layer, kv_head * self.max_ctx + pos,
-                                                buf, hd))
-        return torch.tensor(list(buf), dtype=torch.float32)
+            _lib.check(self._lib.lsk_debug_read(self._h, what, layer, kv_head * self.max_ctx + pos0,
+                                                buf, count * hd))
+        return torch.frombuffer(buf, dtype=torch.float32).clone().view(count, hd)
 
     def debug_set_page_table(self, pages: Sequence[int]) -> None:
         arr = (C.c_int32 * len(pages))(*[int(p) for p in pages])
