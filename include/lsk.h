@@ -154,6 +154,19 @@ int lsk_round(lsk_engine* e, int32_t d_req, lsk_round_out* out);
  * about EOS exactly as the reference does (:66-67). */
 int lsk_ar_step(lsk_engine* e, int32_t* token_out);
 
+/* Teacher-forced scoring of ids[0..n-1] (2 <= n <= max_ctx), single GPU (tp_size == 1).
+ * For i in 0 .. n-2:
+ *   logprob_out[i] = log softmax(logits after ids[0..i])[ids[i+1]]   (fp32)
+ *   greedy_out[i]  = arg-max token of that row, lowest id on ties    (may be NULL)
+ * exit_layer E in [1, n_layers] runs layers [0, E) and then the final norm and LM head, as the
+ * draft does (forward_early, llama_model_utils.py:271-273); E <= 0 means all layers (forward,
+ * :155-209).  Host pointers.  Synchronous; lsk_last_device_ms gives its device time.  It reuses the
+ * KV pool, so it ends any generation in progress: lsk_round / lsk_ar_step / lsk_debug_forward_rows
+ * return LSK_ERR_STATE until the next lsk_prefill.  It needs neither lsk_begin nor
+ * LSK_FLAG_KEEP_LOGITS; with that flag, LSK_DBG_LOGITS afterwards holds the last LM-head slice. */
+int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer,
+              float* logprob_out, int32_t* greedy_out);
+
 /* Queries / debugging (parity tests). */
 int lsk_kv_len(const lsk_engine* e, int32_t* len_out);
 /* Teacher-forced block: the m given ids as one block at positions kv_len .. kv_len+m-1 through
@@ -239,6 +252,11 @@ int lsk_test_attn(const void* q_dev, const void* k_dev, const void* v_dev, int32
 int lsk_test_lmhead_tc(const void* w_bf16_dev, int64_t n, int64_t k, const float* x_f32_dev,
                        const void* norm_w_bf16_dev, float eps, int32_t m, float* logits_dev,
                        float* best_val_dev, int32_t* best_idx_dev, int32_t iters, float* avg_ms_out);
+/* The scoring kernel alone (csrc/misc_kernels.cuh: logprob_rows_kernel) on device buffers: logits
+ * [rows][ld] fp32 with only the first `vocab` columns of each row valid, targets [rows]; writes
+ * logprob [rows] and the per-row arg-max greedy [rows] (nullable). */
+int lsk_test_logprob(const float* logits_dev, int32_t rows, int32_t vocab, int32_t ld,
+                     const int32_t* targets_dev, float* logprob_dev, int32_t* greedy_dev);
 
 #ifdef __cplusplus
 }

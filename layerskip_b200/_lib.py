@@ -94,6 +94,8 @@ SIGNATURES = {
     "lsk_prefill": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
     "lsk_round": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(lsk_round_out)]),
     "lsk_ar_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
+    "lsk_score": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32,
+                            C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
     "lsk_kv_len": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "lsk_debug_forward_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
     "lsk_debug_read": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64,
@@ -119,6 +121,8 @@ SIGNATURES = {
     "lsk_test_lmhead_tc": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                      C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_int32, C.POINTER(C.c_float)]),
+    "lsk_test_logprob": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                   C.c_void_p]),
 }
 
 _lib = None

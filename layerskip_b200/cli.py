@@ -57,6 +57,14 @@ class GenerateArguments:              # generate.py:32-39
     streamer: str = "standard"        # none | standard | speculative
 
 
+@dataclass
+class ScoreArguments:
+    exit_layers: str = "4,8,16,-1"    # comma-separated; -1 (or any value <= 0) = full depth
+    # synthetic dataset only: extend each prompt by this many tokens of the model's own full-depth
+    # greedy output, so the scored text is one the full model finds likely (0 = prompts only)
+    continuation_len: int = 64
+
+
 def parse_model_args(text: Optional[str]) -> Dict[str, Any]:
     """`k=v,k=v` -> dict with bool/int/float coercion (arguments.py:28-55)."""
     out: Dict[str, Any] = {}
@@ -233,6 +241,73 @@ def main_correctness(argv=None):
     print(result)
     spec_strategy.engines.close()
     return result
+
+
+def parse_exit_layers(text: str) -> List[int]:
+    """`"4,8,16,-1"` -> [4, 8, 16, -1]; values <= 0 mean full depth."""
+    return [int(t) for t in text.split(",") if t.strip()]
+
+
+def main_score(argv=None):
+    """Per-exit-layer quality of the early-exit sub-model (layers < E + shared norm and head) in one
+    teacher-forced pass per sequence: mean NLL per token and perplexity, greedy accuracy (arg-max
+    == next token), agreement with full depth (arg-max at E == arg-max at full depth: what greedy
+    self-speculation accepts), and scored tokens per second of device time."""
+    if argv is not None:
+        sys.argv = [sys.argv[0]] + list(argv)
+    args, bargs, sargs = parse(Arguments, BenchmarkArguments, ScoreArguments)
+    if bargs.dataset != "synthetic":
+        raise NotImplementedError("only --dataset synthetic is available offline")
+    exits = parse_exit_layers(sargs.exit_layers)
+    positive = [e for e in exits if e > 0]
+    # alpha damping (--model_args alpha=...) starts at the shallowest exit layer
+    model, _tok, margs = load_model_and_tokenizer(args, min(positive) if positive else -1)
+    arch = model.arch
+    if any(e > arch.layers for e in exits):
+        raise ValueError(f"--exit_layers {sargs.exit_layers}: the model has {arch.layers} layers")
+    from .engine import Engine
+    cont = max(0, sargs.continuation_len)
+    max_ctx = max(int(margs.get("max_ctx", 0)), bargs.prompt_len + cont + 2)
+    eng = Engine(arch, max_ctx=max_ctx)
+    eng.load_model(model)
+    texts = []
+    for p in synthetic_prompts(arch.vocab, bargs.num_samples or 8, bargs.prompt_len):
+        if cont:
+            eng.begin(-1, cont, [])
+            eng.prefill(p)
+            p = p + [eng.ar_step() for _ in range(cont)]
+        texts.append(p)
+    full = {}
+    for i, ids in enumerate(texts):
+        full[i] = eng.score(ids, -1)[1]
+    results = []
+    for e in exits:
+        lp_all, hit, agree, ms = [], 0, 0, 0.0
+        for i, ids in enumerate(texts):
+            lp, greedy = eng.score(ids, e)
+            ms += eng.last_device_ms
+            lp_all.append(lp.to(torch.float64))
+            hit += int((greedy == torch.tensor(ids[1:])).sum())
+            agree += int((greedy == full[i]).sum())
+        lp = torch.cat(lp_all)
+        n_tok = lp.numel()
+        nll = float(-lp.mean())
+        results.append({"exit_layer": e if e > 0 else arch.layers, "mean_nll": nll,
+                        "perplexity": float(torch.exp(torch.tensor(nll, dtype=torch.float64))),
+                        "greedy_accuracy": hit / n_tok, "agreement_with_full": agree / n_tok,
+                        "scored_tokens": n_tok, "device_ms": ms,
+                        "tokens_per_second": n_tok / (ms / 1e3) if ms > 0 else None})
+    eng.close()
+    print(f"{'exit':>5} {'nll/token':>10} {'perplexity':>12} {'greedy acc':>11} {'agree full':>11} {'tokens/s':>11}")
+    for r in results:
+        print(f"{r['exit_layer']:>5} {r['mean_nll']:>10.4f} {r['perplexity']:>12.2f} {r['greedy_accuracy']:>11.4f} "
+              f"{r['agreement_with_full']:>11.4f} {r['tokens_per_second'] or 0:>11.0f}")
+    os.makedirs(args.output_dir, exist_ok=True)
+    path = os.path.join(args.output_dir, f"score_{time.strftime('%Y%m%d_%H%M%S')}.json")
+    with open(path, "w") as f:
+        json.dump({"args": vars(args), "benchmark_arguments": vars(bargs), "score_arguments": vars(sargs),
+                   "results": results}, f, indent=1)
+    return results
 
 
 class _PrintStreamer:

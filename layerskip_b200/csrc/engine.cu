@@ -151,6 +151,8 @@ struct lsk_engine {
   int* rank_idx = nullptr;
   int* d_zero = nullptr;
   int* d_prompt = nullptr;             // [max_ctx] prompt ids
+  float* score_lp = nullptr;           // lsk_score: [max_pos] log-probabilities (allocated on first use)
+  int* score_greedy = nullptr;         // lsk_score: [max_pos] arg-max ids
   DevState* state = nullptr;
   GenParams* gen_dev = nullptr;
   RoundResult* res_host = nullptr;     // mapped pinned
@@ -618,7 +620,10 @@ static int launch_prompt_attention(lsk_engine* e, const __nv_bfloat16* q, int q_
   return LSK_OK;
 }
 
-static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m) {
+// Layers [0, n_run) run on the chunk.  The prompt pass (complete = false) stops the last of them
+// once its K/V rows are written; scoring (complete = true) runs it to the end and folds the pending
+// row-parallel partials into hidden_p, which then holds the residual rows the LM head reads.
+static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool complete) {
   const lsk_config& c = e->cfg;
   const bool tp = c.tp_size > 1;
   e->cur_class = CLS_MISC;
@@ -643,7 +648,7 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m) {
     pend = e->tp_buf_p; n_pend = 1;
     return LSK_OK;
   };
-  for (int li = 0; li < c.n_layers; ++li) {
+  for (int li = 0; li < n_run; ++li) {
     LayerWeights& L = e->layers[li];
     __nv_bfloat16* kp = e->kpool + (size_t)li * e->pool_layer_elems;
     __nv_bfloat16* vp = e->vpool + (size_t)li * e->pool_layer_elems;
@@ -661,7 +666,7 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m) {
     }
     // the prompt pass has no LM head (the reference discards those logits): once the last layer's
     // K/V rows are written nothing downstream is needed
-    if (li + 1 == c.n_layers) break;
+    if (li + 1 == n_run && !complete) break;
     e->cur_class = CLS_ATTN;
     TRY(launch_prompt_attention(e, e->q_p, e->q_rows, e->attn_c, kp, vp, e->page_table, e->d_zero, c0, m,
                                 e->group, e->kv_heads_l, c.head_dim));
@@ -690,6 +695,11 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m) {
       TRY(launch_prefill_gemm<PF_EPI_STORE>(e, a));
       TRY(after_row_parallel(ks_d));
     }
+  }
+  if (complete) {   // residual update only (dst = nullptr): the final norm is the LM head's prologue
+    e->cur_class = CLS_MISC;
+    CU(launch(e, rms_canon_kernel, dim3(m), dim3(256), 0, e->hidden_p, c.hidden, pend, n_pend, part_stride,
+              (const __nv_bfloat16*)e->final_norm, c.rms_eps, c.hidden, (unsigned char*)nullptr));
   }
   return LSK_OK;
 }
@@ -732,6 +742,24 @@ static int emit_ar_commit(lsk_engine* e, int seq) {
   return LSK_OK;
 }
 
+// Final RMSNorm + the mma.sync LM head on M fp32 residual rows at x (row stride hidden): arg-max
+// candidates into cand_*, and the logits rows when `logits` is set.
+static int launch_lm_head_gemm(lsk_engine* e, const float* x, int M, float* logits, const void* after_W = nullptr,
+                               size_t after_bytes = 0) {
+  const lsk_config& c = e->cfg;
+  GemmArgs a{};
+  a.W = reinterpret_cast<const uint4*>(e->lm_head);
+  a.M = M;
+  a.x_f32 = x; a.x_ld = c.hidden;
+  a.norm_w = e->final_norm; a.eps = c.rms_eps;
+  a.logits = logits; a.logits_ld = e->vocab_l_pad;
+  a.n_valid_rows = e->vocab_l; a.vocab_off = e->vocab_off;
+  a.part_val = e->cand_val; a.part_idx = e->cand_idx;
+  a.next_W = after_W;
+  a.next_bytes = after_W ? (after_bytes < e->l2_prefetch_bytes ? after_bytes : e->l2_prefetch_bytes) : 0;
+  return launch_gemm<PRO_RMS, EPI_LMHEAD>(e, e->p_lm, a);
+}
+
 // final RMSNorm + LM head on rows [row0, row0+M): arg-max candidates (and optional logits).
 // (llama_model_utils.py:204-205, 271-273, 386-387).  Afterwards e->cand_* / n_cand() hold one
 // (value, index) per candidate per row.
@@ -743,27 +771,19 @@ static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0, const void* a
   const lsk_config& c = e->cfg;
   const bool ban = e->gen.no_repeat_ngram_size > 0;
   e->cur_class = CLS_LMHEAD;
-  GemmArgs a{};
-  a.W = reinterpret_cast<const uint4*>(e->lm_head);
-  a.M = M;
-  a.x_f32 = e->hidden + (size_t)row0 * c.hidden; a.x_ld = c.hidden;
-  a.norm_w = e->final_norm; a.eps = c.rms_eps;
-  a.logits = (e->keep_logits || e->gen.sample || ban) ? e->logits : nullptr; a.logits_ld = e->vocab_l_pad;
-  a.n_valid_rows = e->vocab_l; a.vocab_off = e->vocab_off;
-  a.part_val = e->cand_val; a.part_idx = e->cand_idx;
-  a.next_W = after_W;
-  a.next_bytes = after_W ? (after_bytes < e->l2_prefetch_bytes ? after_bytes : e->l2_prefetch_bytes) : 0;
+  const float* x = e->hidden + (size_t)row0 * c.hidden;
+  float* logits = (e->keep_logits || e->gen.sample || ban) ? e->logits : nullptr;
   if (e->lm_tc) {
     if (!(e->ablate & (1u << CLS_LMHEAD))) {
       LmHeadTcArgs t{};
       t.W = e->lm_head_tc; t.n_tiles = e->lm_tc_tiles; t.K = c.hidden; t.M = M; t.n_stages = e->lm_tc_stages;
-      t.x_f32 = a.x_f32; t.x_ld = a.x_ld; t.norm_w = a.norm_w; t.eps = a.eps;
-      t.logits = a.logits; t.logits_ld = a.logits_ld; t.n_valid_rows = a.n_valid_rows; t.vocab_off = a.vocab_off;
-      t.part_val = a.part_val; t.part_idx = a.part_idx;
+      t.x_f32 = x; t.x_ld = c.hidden; t.norm_w = e->final_norm; t.eps = c.rms_eps;
+      t.logits = logits; t.logits_ld = e->vocab_l_pad; t.n_valid_rows = e->vocab_l; t.vocab_off = e->vocab_off;
+      t.part_val = e->cand_val; t.part_idx = e->cand_idx;
       CU(launch(e, lmhead_tc_kernel, dim3(e->lm_tc_grid), dim3(kTcThreads),
                 lmhead_tc_smem_bytes(c.hidden, e->lm_tc_stages), t));
     }
-  } else if (!(e->ablate & (1u << CLS_LMHEAD))) TRY((launch_gemm<PRO_RMS, EPI_LMHEAD>(e, e->p_lm, a)));
+  } else if (!(e->ablate & (1u << CLS_LMHEAD))) TRY(launch_lm_head_gemm(e, x, M, logits, after_W, after_bytes));
   e->cur_class = CLS_MISC;
   const float* cv = e->cand_val;
   const int* ci = e->cand_idx;
@@ -1179,7 +1199,8 @@ void lsk_destroy(lsk_engine* e) {
   void* ptrs[] = {e->embed, e->final_norm, e->lm_head, e->lm_head_tc, e->kpool, e->vpool, e->page_table, e->rope,
                   e->hidden, e->qbuf, e->attn_out, e->act, e->tp_buf, e->logits, e->logits_gath, e->logits_full, e->probs_d, e->probs_v, e->samp_scratch, e->cand_val,
                   e->cand_idx, e->gath_val, e->gath_idx, e->ban_val, e->ban_idx, e->rank_val, e->rank_idx,
-                  e->d_zero, e->d_prompt, e->state, e->gen_dev, e->attn_part, e->attn_arrive};
+                  e->d_zero, e->d_prompt, e->state, e->gen_dev, e->attn_part, e->attn_arrive,
+                  e->score_lp, e->score_greedy};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->res_host) cudaFreeHost(e->res_host);
   if (e->ev0) cudaEventDestroy(e->ev0);
@@ -1462,7 +1483,7 @@ int lsk_prefill(lsk_engine* e, const int32_t* ids, int32_t n) {
   if (e->pf_tc && n - 1 > e->max_rows) {
     for (int c0 = 0; c0 < n - 1; c0 += kPfTokens) {
       const int m = (n - 1 - c0) < kPfTokens ? (n - 1 - c0) : kPfTokens;
-      TRY(enqueue_prefill_chunk(e, c0, m));
+      TRY(enqueue_prefill_chunk(e, c0, m, c.n_layers, false));
     }
   } else {
     for (int c0 = 0; c0 < n - 1; c0 += e->max_rows) {
@@ -1591,6 +1612,70 @@ int lsk_debug_forward_rows(lsk_engine* e, const int32_t* ids, int32_t m) {
   if (st != LSK_OK) return st;
   CU(cudaStreamSynchronize(e->stream));
   TRY(peer_check(e));
+  return LSK_OK;
+}
+
+// Teacher-forced scoring (forward / forward_early of llama_model_utils.py:155-276 on the whole
+// sequence): rows 0 .. n-2 through layers [0, E), the final norm and the mma.sync LM head, then per
+// row the log-probability of the next id and the arg-max.  The rows take the prompt pass's route
+// (128-token wgmma chunks, or decode-kernel blocks of max_rows), so their K/V rows overwrite the
+// pool: any generation in progress ends here.
+int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer, float* logprob_out,
+              int32_t* greedy_out) {
+  if (!e || !ids || !logprob_out) return fail(LSK_ERR_INVALID, "null argument");
+  const lsk_config& c = e->cfg;
+  if (c.tp_size > 1) return fail(LSK_ERR_INVALID, "lsk_score needs tp_size 1: tensor-parallel scoring is not supported");
+  if (n < 2) return fail(LSK_ERR_INVALID, "scoring needs at least 2 ids (got %d)", n);
+  if (n > c.max_ctx) return fail(LSK_ERR_CTX, "sequence of %d ids exceeds max_ctx %d", n, c.max_ctx);
+  if (exit_layer > c.n_layers) return fail(LSK_ERR_INVALID, "exit_layer %d > n_layers %d", exit_layer, c.n_layers);
+  for (int i = 0; i < n; ++i)
+    if (ids[i] < 0 || ids[i] >= c.vocab) return fail(LSK_ERR_INVALID, "token id %d out of range", ids[i]);
+  if (!lsk_weights_complete(e)) return fail(LSK_ERR_STATE, "weights not fully loaded");
+  auto alloc0 = [&](void** p, size_t bytes) -> int {
+    if (*p) return LSK_OK;
+    cudaError_t er = cudaMalloc(p, bytes);
+    if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
+    return LSK_OK;
+  };
+  TRY(alloc0((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4));
+  TRY(alloc0((void**)&e->score_lp, (size_t)e->max_pos * 4));
+  TRY(alloc0((void**)&e->score_greedy, (size_t)e->max_pos * 4));
+  const int E = exit_layer <= 0 ? c.n_layers : exit_layer;
+  const int rows = n - 1;
+  e->prefilled = false;
+  e->host_len = 0;
+  // LM head + log softmax on M residual rows at x, which predict ids[r0 + 1 .. r0 + M]
+  auto head = [&](const float* x, int r0, int M) -> int {
+    e->cur_class = CLS_LMHEAD;
+    TRY(launch_lm_head_gemm(e, x, M, e->logits));
+    e->cur_class = CLS_MISC;
+    CU(launch(e, logprob_rows_kernel, dim3(M), dim3(kLogprobThreads), 0, (const float*)e->logits, e->vocab_l_pad,
+              e->vocab_l, (const int*)(e->d_prompt + r0 + 1), e->score_lp + r0, e->score_greedy + r0));
+    return LSK_OK;
+  };
+  CU(cudaEventRecord(e->ev0, e->stream));
+  CU(cudaMemcpyAsync(e->d_prompt, ids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  if (e->pf_tc && rows > e->max_rows) {
+    for (int c0 = 0; c0 < rows; c0 += kPfTokens) {
+      const int m = std::min(rows - c0, kPfTokens);
+      TRY(enqueue_prefill_chunk(e, c0, m, E, true));
+      for (int r0 = 0; r0 < m; r0 += e->max_rows)
+        TRY(head(e->hidden_p + (size_t)r0 * c.hidden, c0 + r0, std::min(m - r0, e->max_rows)));
+    }
+  } else {
+    for (int c0 = 0; c0 < rows; c0 += e->max_rows) {
+      const int m = std::min(rows - c0, e->max_rows);
+      TRY(emit_embed(e, e->d_prompt + c0, e->hidden, m));
+      for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, 0, m, e->d_zero, c0));
+      TRY(head(e->hidden, c0, m));
+    }
+  }
+  CU(cudaEventRecord(e->ev1, e->stream));
+  CU(cudaMemcpyAsync(logprob_out, e->score_lp, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
+  if (greedy_out)
+    CU(cudaMemcpyAsync(greedy_out, e->score_greedy, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
+  CU(cudaStreamSynchronize(e->stream));
+  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
   return LSK_OK;
 }
 
@@ -1988,6 +2073,17 @@ int lsk_test_lmhead_tc(const void* w, int64_t n, int64_t k, const float* x, cons
   CU(cudaEventDestroy(e0));
   CU(cudaEventDestroy(e1));
   cudaFree(canon); cudaFree(cval); cudaFree(cidx);
+  return LSK_OK;
+}
+
+// the scoring kernel alone (unit test): logits [rows][ld] fp32, the first `vocab` columns valid
+int lsk_test_logprob(const float* logits, int32_t rows, int32_t vocab, int32_t ld, const int32_t* targets,
+                     float* logprob, int32_t* greedy) {
+  if (!logits || !targets || !logprob || rows < 1 || vocab < 1 || ld < vocab)
+    return fail(LSK_ERR_INVALID, "bad log-probability test shape");
+  logprob_rows_kernel<<<rows, kLogprobThreads>>>(logits, ld, vocab, (const int*)targets, logprob, (int*)greedy);
+  CU(cudaGetLastError());
+  CU(cudaDeviceSynchronize());
   return LSK_OK;
 }
 

@@ -363,4 +363,58 @@ argmax_rows_kernel(const float* __restrict__ logits, int ld, int v_local, int vo
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// Teacher-forced scoring: per logits row, log softmax at the target id and the arg-max (lowest
+// id wins ties).  One CTA per row, one pass over the `vocab` valid columns (pad columns
+// [vocab, ld) are never read): every thread keeps a running (max m, sum s of exp(v - m)) and its
+// best (value, id); threads merge by a fixed xor tree, warps in index order, so the result is
+// bit-reproducible.  logprob = logit[target] - (m + log s), with expf / logf (not the intrinsics).
+// ---------------------------------------------------------------------------------------
+constexpr int kLogprobThreads = 512;
+
+__device__ __forceinline__ void lse_merge(float& m, float& s, float om, float os) {
+  const float nm = fmaxf(m, om);
+  if (nm == -INFINITY) return;                                   // both empty
+  s = (m == -INFINITY ? 0.f : s * expf(m - nm)) + (om == -INFINITY ? 0.f : os * expf(om - nm));
+  m = nm;
+}
+
+__global__ void __launch_bounds__(kLogprobThreads)
+logprob_rows_kernel(const float* __restrict__ logits, int ld, int vocab, const int* __restrict__ targets,
+                    float* __restrict__ logprob, int* __restrict__ greedy) {
+  __shared__ float s_m[kLogprobThreads / 32], s_s[kLogprobThreads / 32], s_bv[kLogprobThreads / 32];
+  __shared__ int s_bi[kLogprobThreads / 32];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int row = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* lrow = logits + (size_t)row * ld;
+  float m = -INFINITY, s = 0.f, bv = -INFINITY;
+  int bi = 0x7fffffff;
+  for (int c = threadIdx.x; c < vocab; c += kLogprobThreads) {
+    const float v = lrow[c];
+    if (better(v, c, bv, bi)) { bv = v; bi = c; }
+    if (v == -INFINITY) continue;
+    if (v > m) { s = s * expf(m - v) + 1.f; m = v; }             // expf(-inf) = 0 on the first element
+    else s += expf(v - m);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, m, o), os = __shfl_xor_sync(0xffffffffu, s, o);
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    lse_merge(m, s, om, os);
+    if (better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+  }
+  if (lane == 0) { s_m[warp] = m; s_s[warp] = s; s_bv[warp] = bv; s_bi[warp] = bi; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kLogprobThreads / 32; ++w) {
+      lse_merge(m, s, s_m[w], s_s[w]);
+      if (better(s_bv[w], s_bi[w], bv, bi)) { bv = s_bv[w]; bi = s_bi[w]; }
+    }
+    logprob[row] = lrow[targets[row]] - (m + logf(s));
+    if (greedy != nullptr) greedy[row] = bi;
+  }
+}
+
 }  // namespace lsk

@@ -206,6 +206,46 @@ class Engine:
             _lib.check(self._lib.lsk_ar_step(self._h, C.byref(tok)))
         return tok.value
 
+    # ------------------------------------------------------------------ scoring
+    def score(self, ids: Sequence[int], exit_layer: int = -1) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Teacher-forced pass over `ids` (2 <= len(ids) <= max_ctx) through layers < exit_layer
+        (all layers when exit_layer <= 0), the final norm and the LM head.  Returns
+        (logprobs float32[n-1], greedy int64[n-1]): entry i is the log-probability of ids[i+1] and
+        the arg-max token after ids[0..i].  Ends any generation in progress (the next round needs
+        a new prefill)."""
+        n = len(ids)
+        arr = (C.c_int32 * max(n, 1))(*[int(t) for t in ids])
+        lp = (C.c_float * max(n - 1, 1))()
+        gr = (C.c_int32 * max(n - 1, 1))()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_score(self._h, arr, n, int(exit_layer), lp, gr))
+        logprobs = torch.frombuffer(lp, dtype=torch.float32).clone()[:n - 1]
+        greedy = torch.frombuffer(gr, dtype=torch.int32).clone()[:n - 1].to(torch.int64)
+        return logprobs, greedy
+
+    def loglikelihood(self, context: Sequence[int], continuation: Sequence[int],
+                      exit_layer: int = -1) -> Tuple[float, bool]:
+        """Log-likelihood of `continuation` following `context`, and whether greedy decoding from
+        the context would have produced exactly the continuation.
+
+        The two parts are joined and, when longer than max_ctx, the oldest tokens are dropped so
+        the last max_ctx remain.  One teacher-forced pass scores every position; the continuation's
+        tokens are the last len(continuation) targets, and their log-probabilities are summed in
+        float64.  Both parts must be non-empty, and at least one token must precede the
+        continuation after truncation (len(continuation) < max_ctx)."""
+        context, continuation = [int(t) for t in context], [int(t) for t in continuation]
+        if not context or not continuation:
+            raise ValueError("context and continuation must both be non-empty")
+        if len(continuation) >= self.max_ctx:
+            raise ValueError(f"a continuation of {len(continuation)} tokens does not fit max_ctx "
+                             f"{self.max_ctx} with at least one context token")
+        ids = (context + continuation)[-self.max_ctx:]
+        logprobs, greedy = self.score(ids, exit_layer)
+        k = len(continuation)
+        total = float(logprobs[-k:].to(torch.float64).sum())
+        is_greedy = bool(greedy[-k:].tolist() == continuation)
+        return total, is_greedy
+
     # ------------------------------------------------------------------ introspection
     @property
     def kv_len(self) -> int:

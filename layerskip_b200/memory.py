@@ -18,9 +18,12 @@ SM_COUNT = 132                      # H100 SXM: one arg-max candidate slot per S
 
 
 def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling: bool = False,
-                keep_logits: bool = False, lm_head_tc: bool = False, prefill_tc: bool = True) -> Dict[str, int]:
+                keep_logits: bool = False, lm_head_tc: bool = False, prefill_tc: bool = True,
+                scoring: bool = False) -> Dict[str, int]:
     """Bytes the engine allocates on ONE rank.  Keys: weights, embed, lm_head, kv_pool, scratch,
-    total (+ weights_source_peak: the largest single tensor staged on the GPU while loading)."""
+    total (+ weights_source_peak: the largest single tensor staged on the GPU while loading).
+    `scoring` adds what the first `lsk_score` call allocates: the logits rows (unless already
+    there) and one float + one int per position."""
     h, L = arch.hidden, arch.layers
     q_l = arch.heads // tp_size * arch.head_dim
     kv_l = arch.kv_heads // tp_size * arch.head_dim
@@ -56,8 +59,10 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
     scratch += kvh_l * splits * ((arch.heads // arch.kv_heads * 128 + 15) // 16 * 16) * (arch.head_dim + 2) * 4 + kvh_l * 4
     if prefill_tc and h % 64 == 0:
         scratch += 6 * 128 * h * 4 + 128 * q_l * 2 + 16384 * (h // 64 + (q_l + 63) // 64 + (inter_l + 63) // 64)
-    if keep_logits or sampling:
+    if keep_logits or sampling or scoring:
         scratch += MAX_ROWS * vocab_l_pad * 4
+    if scoring:
+        scratch += 2 * max_pos * 4                          # per-position log-probabilities + arg-max ids
     if sampling:
         scratch += (2 * MAX_ROWS + 1) * arch.vocab * 4
         if tp_size > 1:
