@@ -167,6 +167,16 @@ int lsk_ar_step(lsk_engine* e, int32_t* token_out);
 int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer,
               float* logprob_out, int32_t* greedy_out);
 
+/* Teacher-forced scoring of n_seqs sequences in one call, single GPU, wgmma prompt pass required.
+ * Sequence j is ids[offsets[j] .. offsets[j+1]-1], 2 <= length <= max_ctx, offsets[0] == 0.  Outputs
+ * are concatenated in input order: sequence j's (length_j - 1) entries start at offsets[j] - j and
+ * mean exactly what lsk_score's do.  greedy_out may be NULL.  Same state rules as lsk_score.
+ * The rows of all sequences are packed into shared 128-token prompt-pass chunks; every entry is
+ * bit-identical to lsk_score of that sequence alone on the wgmma route (sequences of more than
+ * max_rows + 1 ids). */
+int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
+                    int32_t exit_layer, float* logprob_out, int32_t* greedy_out);
+
 /* Queries / debugging (parity tests). */
 int lsk_kv_len(const lsk_engine* e, int32_t* len_out);
 /* Teacher-forced block: the m given ids as one block at positions kv_len .. kv_len+m-1 through

@@ -96,6 +96,8 @@ SIGNATURES = {
     "lsk_ar_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "lsk_score": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32,
                             C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
+    "lsk_score_batch": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                  C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
     "lsk_kv_len": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "lsk_debug_forward_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
     "lsk_debug_read": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64,

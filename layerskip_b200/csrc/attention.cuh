@@ -58,6 +58,15 @@ struct AttnArgs {
   unsigned int* arrive;        // [n_kv_heads] splits done; zero between launches (the merger resets it)
 };
 
+// Piece grid (attn_piece_kernel): blockIdx.z selects pieces[z] = (chunk row of its first query row,
+// rows, position of that row, first logical page of its page-table view).  q, the canonical output
+// and the partials are addressed by chunk row; AttnArgs::M is the largest piece's rows,
+// AttnArgs::arrive holds [pieces][n_kv_heads] counters.
+struct AttnPieces {
+  const int4* pieces;
+  int part_rows;               // row stride of AttnArgs::part: rows_pad of a whole 128-row chunk
+};
+
 // floats of AttnArgs::part for a launch
 __host__ inline size_t attn_part_floats(int n_kv_heads, int n_splits, int rows_pad, int hd) {
   return (size_t)n_kv_heads * n_splits * rows_pad * (hd + 2);
@@ -93,7 +102,7 @@ __device__ __forceinline__ void team_sync() {
 // bound on the number of splits: with SP <= 4 every value (4 (m, l) pairs + 16 float4) is requested
 // up front — ONE round trip instead of a chain of five; same arithmetic in the same order either way.
 template <int HD, int SP, typename FML, typename FO>
-__device__ __forceinline__ void merge_splits_write(const AttnArgs& a, int kvh, int row, int dseg,
+__device__ __forceinline__ void merge_splits_write(const AttnArgs& a, int kvh, int row, int dseg, int tok0,
                                                    FML ml, FO o) {
   float ms[SP], ls[SP];
 #pragma unroll
@@ -157,7 +166,7 @@ __device__ __forceinline__ void merge_splits_write(const AttnArgs& a, int kvh, i
     }
   }
   const float inv = 1.f / ll;
-  const int tok = row / a.group, hq = kvh * a.group + row % a.group;
+  const int tok = tok0 + row / a.group, hq = kvh * a.group + row % a.group;
   if (a.out_canon) {           // two 16-byte chunks of the O projection's B operand
     unsigned char* base = reinterpret_cast<unsigned char*>(a.out);
 #pragma unroll
@@ -177,9 +186,11 @@ __device__ __forceinline__ void merge_splits_write(const AttnArgs& a, int kvh, i
     *reinterpret_cast<uint32_t*>(op + i) = pack_bf16x2(acc[i] * inv, acc[i + 1] * inv);
 }
 
-template <int HD>
-__global__ void __launch_bounds__(kAttnThreads)
-attn_split_kernel(const AttnArgs a) {
+// PIECES: one launch covers several independent query pieces (packed scoring); blockIdx.z selects
+// the piece, whose rows, positions, page-table view and partials rows come from a.pieces.  A row's
+// arithmetic is the same as in a launch of its own.
+template <int HD, bool PIECES>
+__device__ __forceinline__ void attn_split_body(const AttnArgs& a, const AttnPieces& pz) {
   constexpr int KS = HD / 16;                   // k steps of Q.K^T
   constexpr int DT = HD / 8;                    // n8 tiles of the output
   constexpr int CH = HD / 8;                    // 16-byte chunks per K/V row
@@ -198,6 +209,13 @@ attn_split_kernel(const AttnArgs a) {
   const int kvh = blockIdx.x, split = blockIdx.y;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
+  // this CTA's query rows: the whole launch, or piece blockIdx.z (chunk row tok0)
+  const int4 pc = PIECES ? pz.pieces[blockIdx.z] : make_int4(0, 0, 0, 0);
+  const int tok0 = pc.x;
+  const int M = PIECES ? pc.y : a.M;
+  const int pos_off = PIECES ? pc.z : a.pos_off;
+  const int* page_table = PIECES ? a.page_table + pc.w : a.page_table;
+  const __nv_bfloat16* qb = PIECES ? a.q + (size_t)tok0 * a.q_ld : a.q;
 
   if (tid == 0) {
     for (int s = 0; s < kAttnStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
@@ -209,11 +227,11 @@ attn_split_kernel(const AttnArgs a) {
   // ---- everything below up to pdl_wait() reads only data that is constant while the enclosing
   // graph runs: the committed length, the page table, and K/V rows below the committed length
   const int len0 = *a.base_len;
-  const int base = len0 + a.pos_off;                 // position of token row 0
-  const int n_keys = base + a.M;                     // keys visible to the last row
+  const int base = len0 + pos_off;                   // position of token row 0
+  const int n_keys = base + M;                       // keys visible to the last row
   const int n_kgroups = (n_keys + kKeyGroup - 1) / kKeyGroup;
   const int n_mine = split < n_kgroups ? (n_kgroups - split + a.n_splits - 1) / a.n_splits : 0;
-  const int R = a.group * a.M;                       // real query rows (token-major)
+  const int R = a.group * M;                         // real query rows (token-major)
   const int n_rb = (R + 15) / 16;
   const bool reload = a.reload_per_rb != 0 || n_mine > kAttnStages;   // K/V re-fetched per row block
   int issued = 0;                                                    // (thread 0) items handed to the TMA engine
@@ -223,7 +241,7 @@ attn_split_kernel(const AttnArgs a) {
     const int kg = split + j * a.n_splits;
     const int st = item % kAttnStages;
     mbar_wait(&empty_bar[st], ((item / kAttnStages) & 1) ^ 1);
-    const int page = a.page_table[kg];               // kKeyGroup == kPageTokens
+    const int page = page_table[kg];                 // kKeyGroup == kPageTokens
     const size_t blk = (size_t)(page * a.n_kv_heads + kvh) * kPageTokens * HD;
     unsigned char* dst = stages + (size_t)st * kStageBytes;
     mbar_arrive_expect_tx(&full_bar[st], kStageBytes);
@@ -248,8 +266,8 @@ attn_split_kernel(const AttnArgs a) {
       const int r0 = rb * 16 + g, r1 = r0 + 8;
       const __nv_bfloat16* q0 = nullptr;
       const __nv_bfloat16* q1 = nullptr;
-      if (r0 < R) q0 = a.q + (size_t)(r0 / a.group) * a.q_ld + (kvh * a.group + r0 % a.group) * HD;
-      if (r1 < R) q1 = a.q + (size_t)(r1 / a.group) * a.q_ld + (kvh * a.group + r1 % a.group) * HD;
+      if (r0 < R) q0 = qb + (size_t)(r0 / a.group) * a.q_ld + (kvh * a.group + r0 % a.group) * HD;
+      if (r1 < R) q1 = qb + (size_t)(r1 / a.group) * a.q_ld + (kvh * a.group + r1 % a.group) * HD;
 #pragma unroll
       for (int k = 0; k < KS; ++k) {
         qf[k][0] = q0 ? *reinterpret_cast<const uint32_t*>(q0 + k * 16 + 2 * t) : 0u;
@@ -414,14 +432,19 @@ attn_split_kernel(const AttnArgs a) {
   }
 
   // ---- publish this split's partial rows (same layout as po / pml)
-  const size_t part_floats = (size_t)a.rows_pad * (HD + 2);
+  // (a piece's rows sit at chunk row tok0 of partials laid out for a whole chunk, part_rows rows)
+  const int prows = PIECES ? pz.part_rows : a.rows_pad;
+  const size_t part_floats = (size_t)prows * (HD + 2);
+  const size_t o_off = PIECES ? (size_t)a.group * tok0 * HD : 0;
+  const size_t ml_off = (size_t)prows * HD + (PIECES ? (size_t)a.group * tok0 * 2 : 0);
+  unsigned int* arrive = PIECES ? a.arrive + (size_t)blockIdx.z * a.n_kv_heads : a.arrive;
   float* gp = a.part + (size_t)(kvh * a.n_splits + split) * part_floats;
   for (int i = tid; i < R * (HD / 4); i += kAttnThreads)
-    reinterpret_cast<float4*>(gp)[i] = reinterpret_cast<const float4*>(po)[i];
-  for (int i = tid; i < 2 * R; i += kAttnThreads) gp[(size_t)a.rows_pad * HD + i] = pml[i];
+    reinterpret_cast<float4*>(gp + o_off)[i] = reinterpret_cast<const float4*>(po)[i];
+  for (int i = tid; i < 2 * R; i += kAttnThreads) gp[ml_off + i] = pml[i];
   __threadfence();
   __syncthreads();
-  if (tid == 0) *last = atomicAdd(&a.arrive[kvh], 1u) == (unsigned)(a.n_splits - 1);
+  if (tid == 0) *last = atomicAdd(&arrive[kvh], 1u) == (unsigned)(a.n_splits - 1);
   __syncthreads();
   if (!*last) return;
 
@@ -431,12 +454,25 @@ attn_split_kernel(const AttnArgs a) {
   const float* hp = a.part + (size_t)kvh * a.n_splits * part_floats;
   for (int it = tid; it < R * SEG; it += kAttnThreads) {
     const int row = it / SEG, dseg = (it % SEG) * 16;
-    auto f_ml = [&](int s) { return hp + s * part_floats + (size_t)a.rows_pad * HD + row * 2; };
-    auto f_o = [&](int s) { return hp + s * part_floats + (size_t)row * HD + dseg; };
-    if (a.n_splits <= 4) merge_splits_write<HD, 4>(a, kvh, row, dseg, f_ml, f_o);
-    else merge_splits_write<HD, kMaxSplits>(a, kvh, row, dseg, f_ml, f_o);
+    auto f_ml = [&](int s) { return hp + s * part_floats + ml_off + row * 2; };
+    auto f_o = [&](int s) { return hp + s * part_floats + o_off + (size_t)row * HD + dseg; };
+    if (a.n_splits <= 4) merge_splits_write<HD, 4>(a, kvh, row, dseg, tok0, f_ml, f_o);
+    else merge_splits_write<HD, kMaxSplits>(a, kvh, row, dseg, tok0, f_ml, f_o);
   }
-  if (tid == 0) a.arrive[kvh] = 0u;   // every split has arrived: ready for the next launch
+  if (tid == 0) arrive[kvh] = 0u;   // every split has arrived: ready for the next launch
+}
+
+template <int HD>
+__global__ void __launch_bounds__(kAttnThreads)
+attn_split_kernel(const AttnArgs a) {
+  attn_split_body<HD, false>(a, AttnPieces{nullptr, 0});
+}
+
+// grid (kv heads, splits, pieces): every piece of a packed prompt-pass chunk in one launch
+template <int HD>
+__global__ void __launch_bounds__(kAttnThreads)
+attn_piece_kernel(const AttnArgs a, const AttnPieces pz) {
+  attn_split_body<HD, true>(a, pz);
 }
 
 }  // namespace lsk

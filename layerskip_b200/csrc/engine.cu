@@ -153,6 +153,8 @@ struct lsk_engine {
   int* d_prompt = nullptr;             // [max_ctx] prompt ids
   float* score_lp = nullptr;           // lsk_score: [max_pos] log-probabilities (allocated on first use)
   int* score_greedy = nullptr;         // lsk_score: [max_pos] arg-max ids
+  int* batch_buf = nullptr;            // lsk_score_batch: [8][max_pos] row ids, targets, row map, pieces of a group
+  unsigned int* piece_arrive = nullptr;  // lsk_score_batch: [128 pieces][kv heads] attention arrival counters
   DevState* state = nullptr;
   GenParams* gen_dev = nullptr;
   RoundResult* res_host = nullptr;     // mapped pinned
@@ -427,29 +429,32 @@ static AttnLaunchPlan plan_attention_launch(int head_dim, int group, int M, int 
 
 // Attention over the paged cache: grid (kv heads, splits), the last split of a head to finish
 // merges; head_dim selects the instantiation, the shared-memory plan depends on (group, M).
+// pz: the piece grid (kv heads, splits, pieces) of attn_piece_kernel, with a.M the largest piece's rows.
 template <int HD>
-static int launch_attention_t(lsk_engine* e, AttnArgs& a) {
+static int launch_attention_t(lsk_engine* e, AttnArgs& a, const AttnPieces* pz, int n_pieces) {
   static std::atomic<uint64_t> configured{0};
-  auto kern = attn_split_kernel<HD>;
   int dev = 0;
   CU(cudaGetDevice(&dev));
   const uint64_t bit = 1ull << (dev & 63);
   if (!(configured.load(std::memory_order_relaxed) & bit)) {
-    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+    CU(cudaFuncSetAttribute(attn_split_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+    CU(cudaFuncSetAttribute(attn_piece_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
     configured.fetch_or(bit, std::memory_order_relaxed);
   }
-  const AttnLaunchPlan lp = plan_attention_launch(HD, a.group, a.M, a.n_kv_heads, a.n_splits, e->attn_stages, e->sm_count);
+  const int grid_z = pz ? n_pieces : 1;
+  const AttnLaunchPlan lp = plan_attention_launch(HD, a.group, a.M, a.n_kv_heads * grid_z, a.n_splits, e->attn_stages,
+                                                  e->sm_count);
   const AttnSmemPlan& sp = lp.sp;
   a.n_stages = lp.stages;
   if (!lp.ok)
     return fail(LSK_ERR_INVALID, "attention: %d query rows per kv head do not fit shared memory", a.group * a.M);
   a.rows_pad = (a.group * a.M + 15) / 16 * 16;
   a.merge_off = sp.merge_off; a.part_off = sp.part_off; a.reload_per_rb = sp.reload_per_rb;
-  if (attn_part_floats(a.n_kv_heads, a.n_splits, a.rows_pad, HD) > e->attn_part_cap)
+  if (attn_part_floats(a.n_kv_heads, a.n_splits, pz ? pz->part_rows : a.rows_pad, HD) > e->attn_part_cap)
     return fail(LSK_ERR_INVALID, "attention: %d query rows per kv head exceed the partials buffer", a.group * a.M);
-  a.part = e->attn_part; a.arrive = e->attn_arrive;
+  a.part = e->attn_part; a.arrive = pz ? e->piece_arrive : e->attn_arrive;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(a.n_kv_heads, a.n_splits);
+  cfg.gridDim = dim3(a.n_kv_heads, a.n_splits, grid_z);
   cfg.blockDim = dim3(kAttnThreads);
   // a grid that fits one wave gets a whole SM per CTA (> half of the SM's shared memory): the
   // CTAs then spread over the SMs instead of sharing a few SMs' load bandwidth
@@ -462,24 +467,27 @@ static int launch_attention_t(lsk_engine* e, AttnArgs& a) {
   cfg.numAttrs = e->use_pdl ? 1 : 0;
   e->launches += 1;
   e->capture_launches += 1;
+  auto go = [&]() {
+    return pz ? cudaLaunchKernelEx(&cfg, attn_piece_kernel<HD>, a, *pz) : cudaLaunchKernelEx(&cfg, attn_split_kernel<HD>, a);
+  };
   if (!e->profiling) {
-    CU(cudaLaunchKernelEx(&cfg, kern, a));
+    CU(go());
   } else {
     cudaEvent_t ea, eb;
     cudaEventCreate(&ea); cudaEventCreate(&eb);
     cudaEventRecord(ea, e->stream);
-    cudaError_t err = cudaLaunchKernelEx(&cfg, kern, a);
+    cudaError_t err = go();
     cudaEventRecord(eb, e->stream);
     e->prof_events.push_back({e->cur_class, {ea, eb}});
     CU(err);
   }
   return LSK_OK;
 }
-static int launch_attention(lsk_engine* e, AttnArgs& a, int head_dim) {
+static int launch_attention(lsk_engine* e, AttnArgs& a, int head_dim, const AttnPieces* pz = nullptr, int n_pieces = 0) {
   switch (head_dim) {
-    case 128: return launch_attention_t<128>(e, a);
-    case 64: return launch_attention_t<64>(e, a);
-    case 32: return launch_attention_t<32>(e, a);
+    case 128: return launch_attention_t<128>(e, a, pz, n_pieces);
+    case 64: return launch_attention_t<64>(e, a, pz, n_pieces);
+    case 32: return launch_attention_t<32>(e, a, pz, n_pieces);
     default: return fail(LSK_ERR_INVALID, "head_dim %d unsupported (32, 64 or 128)", head_dim);
   }
 }
@@ -600,12 +608,15 @@ static int launch_prefill_gemm(lsk_engine* e, PrefillGemmArgs& a) {
 // that the O projection of prefill_tc.cuh reads.  One launch per m_attn rows: as many as fit the
 // attention kernel's shared-memory plan (a multiple of 16, so the canonical swizzle of row r0 + j
 // equals that of row j).
+static int prompt_attn_rows(int head_dim, int group) {
+  for (int cand = kPfTokens; cand >= 16; cand -= 16)
+    if (attn_smem_plan(head_dim, group, cand, 2).total <= (size_t)kSmemMax) return cand;
+  return 16;
+}
 static int launch_prompt_attention(lsk_engine* e, const __nv_bfloat16* q, int q_ld, unsigned char* out_canon,
                                    const __nv_bfloat16* kp, const __nv_bfloat16* vp, const int* page_table,
                                    const int* zero, int c0, int m, int group, int n_kv_heads, int head_dim) {
-  int m_attn = 16;
-  for (int cand = kPfTokens; cand >= 16; cand -= 16)
-    if (attn_smem_plan(head_dim, group, cand, 2).total <= (size_t)kSmemMax) { m_attn = cand; break; }
+  const int m_attn = prompt_attn_rows(head_dim, group);
   for (int r0 = 0; r0 < m; r0 += m_attn) {
     AttnArgs a{};
     a.q = q + (size_t)r0 * q_ld; a.q_ld = q_ld;
@@ -620,15 +631,27 @@ static int launch_prompt_attention(lsk_engine* e, const __nv_bfloat16* q, int q_
   return LSK_OK;
 }
 
+// A chunk of rows from several sequences (lsk_score_batch), device pointers at the chunk's first row:
+// ids, per-row (position, first logical page), and the chunk's attention pieces (AttnPieces::pieces).
+struct PackedChunk {
+  const int* ids;
+  const int2* row_map;
+  const int4* pieces;
+  int n_pieces, max_piece_rows;
+};
+
 // Layers [0, n_run) run on the chunk.  The prompt pass (complete = false) stops the last of them
 // once its K/V rows are written; scoring (complete = true) runs it to the end and folds the pending
 // row-parallel partials into hidden_p, which then holds the residual rows the LM head reads.
-static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool complete) {
+// With `pk` the rows are a packed chunk: ids, positions and pages come from it, and one piece-grid
+// attention launch per layer covers every piece (c0 is then unused).
+static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool complete,
+                                 const PackedChunk* pk = nullptr) {
   const lsk_config& c = e->cfg;
   const bool tp = c.tp_size > 1;
   e->cur_class = CLS_MISC;
   CU(launch(e, embed_tokens_kernel, dim3(m), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
-            (const int*)(e->d_prompt + c0), e->hidden_p, c.hidden));
+            pk ? pk->ids : (const int*)(e->d_prompt + c0), e->hidden_p, c.hidden));
   // row-parallel GEMMs (O / down): hidden / 128 feature tiles are too few to keep the SMs streaming
   // -> split K; the partial tiles are summed (fixed order) by the next rms_canon_kernel
   const int ks_o = std::max(1, std::min(std::min(4, e->kst_q), e->sm_count / e->pf_t_h));
@@ -662,14 +685,30 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool c
       a.q_out = e->q_p; a.q_ld = e->q_rows; a.kpool = kp; a.vpool = vp; a.page_table = e->page_table;
       a.pos0 = c0; a.rope = e->rope; a.head_dim = c.head_dim;
       a.q_rows = e->q_rows; a.kv_rows = e->kv_rows; a.n_kv_heads = e->kv_heads_l;
-      TRY(launch_prefill_gemm<PF_EPI_QKV>(e, a));
+      if (pk) {
+        a.row_map = pk->row_map;
+        TRY(launch_prefill_gemm<PF_EPI_QKV_MAP>(e, a));
+      } else {
+        TRY(launch_prefill_gemm<PF_EPI_QKV>(e, a));
+      }
     }
     // the prompt pass has no LM head (the reference discards those logits): once the last layer's
     // K/V rows are written nothing downstream is needed
     if (li + 1 == n_run && !complete) break;
     e->cur_class = CLS_ATTN;
-    TRY(launch_prompt_attention(e, e->q_p, e->q_rows, e->attn_c, kp, vp, e->page_table, e->d_zero, c0, m,
-                                e->group, e->kv_heads_l, c.head_dim));
+    if (pk) {
+      AttnArgs a{};
+      a.q = e->q_p; a.q_ld = e->q_rows;
+      a.out = reinterpret_cast<__nv_bfloat16*>(e->attn_c); a.out_canon = 1;
+      a.kpool = kp; a.vpool = vp; a.page_table = e->page_table; a.base_len = e->d_zero;
+      a.M = pk->max_piece_rows; a.group = e->group; a.n_kv_heads = e->kv_heads_l; a.n_splits = e->n_splits;
+      a.scale = 1.0f / sqrtf((float)c.head_dim);
+      const AttnPieces pz{pk->pieces, (e->group * kPfTokens + 15) / 16 * 16};
+      TRY(launch_attention(e, a, c.head_dim, &pz, pk->n_pieces));
+    } else {
+      TRY(launch_prompt_attention(e, e->q_p, e->q_rows, e->attn_c, kp, vp, e->page_table, e->d_zero, c0, m,
+                                  e->group, e->kv_heads_l, c.head_dim));
+    }
     e->cur_class = CLS_O;
     {
       PrefillGemmArgs a{};
@@ -1109,6 +1148,7 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
     CU(cudaFuncSetAttribute(prefill_gemm_tc_kernel<PF_EPI_QKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
     CU(cudaFuncSetAttribute(prefill_gemm_tc_kernel<PF_EPI_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
     CU(cudaFuncSetAttribute(prefill_gemm_tc_kernel<PF_EPI_SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
+    CU(cudaFuncSetAttribute(prefill_gemm_tc_kernel<PF_EPI_QKV_MAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
   }
   TRY(alloc((void**)&e->embed, (size_t)c.vocab * h * 2));
   TRY(alloc((void**)&e->final_norm, h * 2));
@@ -1200,7 +1240,7 @@ void lsk_destroy(lsk_engine* e) {
                   e->hidden, e->qbuf, e->attn_out, e->act, e->tp_buf, e->logits, e->logits_gath, e->logits_full, e->probs_d, e->probs_v, e->samp_scratch, e->cand_val,
                   e->cand_idx, e->gath_val, e->gath_idx, e->ban_val, e->ban_idx, e->rank_val, e->rank_idx,
                   e->d_zero, e->d_prompt, e->state, e->gen_dev, e->attn_part, e->attn_arrive,
-                  e->score_lp, e->score_greedy};
+                  e->score_lp, e->score_greedy, e->batch_buf, e->piece_arrive};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->res_host) cudaFreeHost(e->res_host);
   if (e->ev0) cudaEventDestroy(e->ev0);
@@ -1615,6 +1655,36 @@ int lsk_debug_forward_rows(lsk_engine* e, const int32_t* ids, int32_t m) {
   return LSK_OK;
 }
 
+// Scoring buffers, allocated on the first lsk_score / lsk_score_batch call.
+static int alloc_scoring(lsk_engine* e, bool batch) {
+  auto alloc0 = [&](void** p, size_t bytes) -> int {
+    if (*p) return LSK_OK;
+    cudaError_t er = cudaMalloc(p, bytes);
+    if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
+    return LSK_OK;
+  };
+  TRY(alloc0((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4));
+  TRY(alloc0((void**)&e->score_lp, (size_t)e->max_pos * 4));
+  TRY(alloc0((void**)&e->score_greedy, (size_t)e->max_pos * 4));
+  if (batch && !e->piece_arrive) {
+    TRY(alloc0((void**)&e->batch_buf, (size_t)8 * e->max_pos * 4));
+    TRY(alloc0((void**)&e->piece_arrive, (size_t)kPfTokens * e->kv_heads_l * 4));
+    CU(cudaMemsetAsync(e->piece_arrive, 0, (size_t)kPfTokens * e->kv_heads_l * 4, e->stream));
+  }
+  return LSK_OK;
+}
+
+// LM head + log softmax on M residual rows at x: the log-probabilities of targets[0 .. M) and the
+// arg-max ids go to score_lp / score_greedy from row r on.
+static int enqueue_score_head(lsk_engine* e, const float* x, int M, const int* targets, int r) {
+  e->cur_class = CLS_LMHEAD;
+  TRY(launch_lm_head_gemm(e, x, M, e->logits));
+  e->cur_class = CLS_MISC;
+  CU(launch(e, logprob_rows_kernel, dim3(M), dim3(kLogprobThreads), 0, (const float*)e->logits, e->vocab_l_pad,
+            e->vocab_l, targets, e->score_lp + r, e->score_greedy + r));
+  return LSK_OK;
+}
+
 // Teacher-forced scoring (forward / forward_early of llama_model_utils.py:155-276 on the whole
 // sequence): rows 0 .. n-2 through layers [0, E), the final norm and the mma.sync LM head, then per
 // row the log-probability of the next id and the arg-max.  The rows take the prompt pass's route
@@ -1631,27 +1701,14 @@ int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer, 
   for (int i = 0; i < n; ++i)
     if (ids[i] < 0 || ids[i] >= c.vocab) return fail(LSK_ERR_INVALID, "token id %d out of range", ids[i]);
   if (!lsk_weights_complete(e)) return fail(LSK_ERR_STATE, "weights not fully loaded");
-  auto alloc0 = [&](void** p, size_t bytes) -> int {
-    if (*p) return LSK_OK;
-    cudaError_t er = cudaMalloc(p, bytes);
-    if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
-    return LSK_OK;
-  };
-  TRY(alloc0((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4));
-  TRY(alloc0((void**)&e->score_lp, (size_t)e->max_pos * 4));
-  TRY(alloc0((void**)&e->score_greedy, (size_t)e->max_pos * 4));
+  TRY(alloc_scoring(e, false));
   const int E = exit_layer <= 0 ? c.n_layers : exit_layer;
   const int rows = n - 1;
   e->prefilled = false;
   e->host_len = 0;
-  // LM head + log softmax on M residual rows at x, which predict ids[r0 + 1 .. r0 + M]
+  // M residual rows at x predict ids[r0 + 1 .. r0 + M]
   auto head = [&](const float* x, int r0, int M) -> int {
-    e->cur_class = CLS_LMHEAD;
-    TRY(launch_lm_head_gemm(e, x, M, e->logits));
-    e->cur_class = CLS_MISC;
-    CU(launch(e, logprob_rows_kernel, dim3(M), dim3(kLogprobThreads), 0, (const float*)e->logits, e->vocab_l_pad,
-              e->vocab_l, (const int*)(e->d_prompt + r0 + 1), e->score_lp + r0, e->score_greedy + r0));
-    return LSK_OK;
+    return enqueue_score_head(e, x, M, e->d_prompt + r0 + 1, r0);
   };
   CU(cudaEventRecord(e->ev0, e->stream));
   CU(cudaMemcpyAsync(e->d_prompt, ids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
@@ -1674,6 +1731,102 @@ int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer, 
   CU(cudaMemcpyAsync(logprob_out, e->score_lp, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
   if (greedy_out)
     CU(cudaMemcpyAsync(greedy_out, e->score_greedy, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
+  CU(cudaStreamSynchronize(e->stream));
+  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
+  return LSK_OK;
+}
+
+// Teacher-forced scoring of many sequences on the wgmma prompt pass.  The rows of all sequences
+// (row i of a sequence predicts its id i + 1) are concatenated in input order and cut into 128-row
+// chunks.  A group is a run of sequences whose KV pages fit the pool together: sequence j owns the
+// logical pages [P_j, P_j + ceil((n_j - 1) / 64)), so its keys sit at positions 0 .. n_j - 2 of its
+// own page-table view, where lsk_score puts them, and a sequence's later chunks attend to the K/V
+// rows its earlier chunks wrote.  One upload per group carries the row ids, the targets, the row map
+// (position, first page) and the pieces of every chunk: maximal runs of one sequence's rows inside
+// a chunk, cut to the rows one prompt-attention launch holds.  Every row's arithmetic is that of
+// lsk_score on the same sequence's wgmma route.
+int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs, int32_t exit_layer,
+                    float* logprob_out, int32_t* greedy_out) {
+  if (!e || !ids || !offsets || !logprob_out) return fail(LSK_ERR_INVALID, "null argument");
+  const lsk_config& c = e->cfg;
+  if (c.tp_size > 1)
+    return fail(LSK_ERR_INVALID, "lsk_score_batch needs tp_size 1: tensor-parallel scoring is not supported");
+  if (!e->pf_tc) return fail(LSK_ERR_INVALID, "lsk_score_batch needs the wgmma prompt pass, which this engine does not have");
+  if (n_seqs < 1) return fail(LSK_ERR_INVALID, "n_seqs must be at least 1 (got %d)", n_seqs);
+  if (exit_layer > c.n_layers) return fail(LSK_ERR_INVALID, "exit_layer %d > n_layers %d", exit_layer, c.n_layers);
+  if (offsets[0] != 0) return fail(LSK_ERR_INVALID, "offsets[0] must be 0 (got %d)", offsets[0]);
+  for (int j = 0; j < n_seqs; ++j) {
+    if (offsets[j + 1] <= offsets[j])
+      return fail(LSK_ERR_INVALID, "offsets are not increasing at sequence %d (%d, %d)", j, offsets[j], offsets[j + 1]);
+    const int n = offsets[j + 1] - offsets[j];
+    if (n < 2) return fail(LSK_ERR_INVALID, "sequence %d has %d id: scoring needs at least 2", j, n);
+    if (n > c.max_ctx) return fail(LSK_ERR_CTX, "sequence %d of %d ids exceeds max_ctx %d", j, n, c.max_ctx);
+    for (int i = offsets[j]; i < offsets[j + 1]; ++i)
+      if (ids[i] < 0 || ids[i] >= c.vocab) return fail(LSK_ERR_INVALID, "sequence %d: token id %d out of range", j, ids[i]);
+  }
+  if (!lsk_weights_complete(e)) return fail(LSK_ERR_STATE, "weights not fully loaded");
+  TRY(alloc_scoring(e, true));
+  const int E = exit_layer <= 0 ? c.n_layers : exit_layer;
+  const int m_attn = prompt_attn_rows(c.head_dim, e->group);
+  e->prefilled = false;
+  e->host_len = 0;
+  std::vector<int32_t> up;        // the group's upload: ids [rows], targets [rows], row map [rows][2], pieces [][4]
+  std::vector<int4> pieces;
+  std::vector<int> chunk_first;   // first piece of each chunk, then the piece count
+  CU(cudaEventRecord(e->ev0, e->stream));
+  for (int j = 0, out_row = 0; j < n_seqs;) {
+    int k = j, pages = 0, rows = 0;
+    while (k < n_seqs) {
+      const int nr = offsets[k + 1] - offsets[k] - 1, np = (nr + kPageTokens - 1) / kPageTokens;
+      if (pages + np > e->n_pages) break;
+      pages += np; rows += nr; ++k;
+    }
+    up.assign((size_t)4 * rows, 0);
+    pieces.clear();
+    chunk_first.clear();
+    for (int s = j, r = 0, page = 0; s < k; ++s) {
+      const int32_t* sid = ids + offsets[s];
+      const int nr = offsets[s + 1] - offsets[s] - 1;
+      for (int i = 0; i < nr; ++i) {
+        up[r + i] = sid[i];
+        up[rows + r + i] = sid[i + 1];
+        up[2 * rows + 2 * (r + i)] = i;
+        up[2 * rows + 2 * (r + i) + 1] = page;
+      }
+      for (int i = 0; i < nr;) {
+        const int row = r + i, chunk = row / kPfTokens;
+        const int len = std::min(std::min(nr - i, (chunk + 1) * kPfTokens - row), m_attn);
+        while ((int)chunk_first.size() <= chunk) chunk_first.push_back((int)pieces.size());
+        pieces.push_back(make_int4(row - chunk * kPfTokens, len, i, page));
+        i += len;
+      }
+      r += nr;
+      page += (nr + kPageTokens - 1) / kPageTokens;
+    }
+    chunk_first.push_back((int)pieces.size());
+    up.resize((size_t)4 * rows + 4 * pieces.size());
+    memcpy(up.data() + (size_t)4 * rows, pieces.data(), pieces.size() * sizeof(int4));
+    CU(cudaMemcpyAsync(e->batch_buf, up.data(), up.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    const int* d_ids = e->batch_buf;
+    const int* d_tgt = e->batch_buf + rows;
+    const int2* d_map = reinterpret_cast<const int2*>(e->batch_buf + 2 * rows);
+    const int4* d_pieces = reinterpret_cast<const int4*>(e->batch_buf + 4 * rows);
+    for (int ci = 0, c0 = 0; c0 < rows; ++ci, c0 += kPfTokens) {
+      const int m = std::min(rows - c0, kPfTokens);
+      PackedChunk pk{d_ids + c0, d_map + c0, d_pieces + chunk_first[ci], chunk_first[ci + 1] - chunk_first[ci], 0};
+      for (int p = chunk_first[ci]; p < chunk_first[ci + 1]; ++p) pk.max_piece_rows = std::max(pk.max_piece_rows, pieces[p].y);
+      TRY(enqueue_prefill_chunk(e, c0, m, E, true, &pk));
+      for (int r0 = 0; r0 < m; r0 += e->max_rows)
+        TRY(enqueue_score_head(e, e->hidden_p + (size_t)r0 * c.hidden, std::min(m - r0, e->max_rows), d_tgt + c0 + r0,
+                               c0 + r0));
+    }
+    if (k == n_seqs) CU(cudaEventRecord(e->ev1, e->stream));
+    CU(cudaMemcpyAsync(logprob_out + out_row, e->score_lp, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
+    if (greedy_out)
+      CU(cudaMemcpyAsync(greedy_out + out_row, e->score_greedy, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
+    out_row += rows;
+    j = k;
+  }
   CU(cudaStreamSynchronize(e->stream));
   CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
   return LSK_OK;

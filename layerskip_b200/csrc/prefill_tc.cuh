@@ -45,7 +45,9 @@ constexpr int kPfTokens = 128;                 // UMMA N: token rows per prefill
 constexpr int kPfStageBytes = 2 * kTcStageBytes;   // A stage + B stage
 constexpr int kPfMaxStages = 6;
 
-enum { PF_EPI_QKV = 0, PF_EPI_STORE = 2, PF_EPI_SILU = 3 };
+// PF_EPI_QKV_MAP: the QKV epilogue with per-row positions and page-table views (row_map): token
+// rows of several sequences packed into one chunk
+enum { PF_EPI_QKV = 0, PF_EPI_STORE = 2, PF_EPI_SILU = 3, PF_EPI_QKV_MAP = 4 };
 
 struct PrefillGemmArgs {
   const unsigned char* W;      // canonical weights [n_tiles][n_kst][16 KiB]
@@ -71,6 +73,7 @@ struct PrefillGemmArgs {
   const float2* rope;
   int head_dim;
   int q_rows, kv_rows, n_kv_heads;
+  const int2* row_map;         // QKV_MAP: per token row (position, first logical page of its page-table view)
 };
 
 // + 1 KiB: the ring is aligned up to 1024 bytes inside the dynamic shared memory
@@ -271,7 +274,7 @@ prefill_gemm_tc_kernel(const PrefillGemmArgs a) {
           *reinterpret_cast<__nv_bfloat16*>(a.act_canon + canon_offset(tok, kidx)) = __float2bfloat16_rn(sg * u);
         }
       }
-    } else {  // PF_EPI_QKV
+    } else {  // PF_EPI_QKV, PF_EPI_QKV_MAP
       // a pair never straddles q / k / v or a head (all are multiples of head_dim >= 32 rows)
       const int HD = a.head_dim, half = HD >> 1;
       const bool is_q = prow < a.q_rows, is_k = !is_q && prow < a.q_rows + a.kv_rows;
@@ -287,7 +290,13 @@ prefill_gemm_tc_kernel(const PrefillGemmArgs a) {
         if (j & 2) continue;
         const int tok = 8 * (j >> 2) + 2 * (lane & 3) + (j & 1);
         if (tok >= a.M || !valid_lo) continue;
-        const int pos = a.pos0 + tok;
+        int pos = a.pos0 + tok;
+        const int* page_table = a.page_table;
+        if (EPI == PF_EPI_QKV_MAP) {
+          const int2 rm = a.row_map[tok];
+          pos = rm.x;
+          page_table += rm.y;
+        }
         // lower row of the pair holds x[d] (lo), upper row x[d + half] (hi):
         //   out_lo = lo cos - hi sin,  out_hi = hi cos + lo sin   (rotate_half, modeling_llama.py:138-168)
         const float lo = d[j], hi = d[j + 2];
@@ -302,7 +311,7 @@ prefill_gemm_tc_kernel(const PrefillGemmArgs a) {
           qo[dd_lo] = __float2bfloat16_rn(out_lo);
           qo[dd_hi] = __float2bfloat16_rn(out_hi);
         } else {
-          const int page = a.page_table[pos >> 6];
+          const int page = page_table[pos >> 6];
           pool[kv_elem_offset(HD, page, a.n_kv_heads, head, pos & 63, dd_lo)] = __float2bfloat16_rn(out_lo);
           if (valid_hi) pool[kv_elem_offset(HD, page, a.n_kv_heads, head, pos & 63, dd_hi)] = __float2bfloat16_rn(out_hi);
         }

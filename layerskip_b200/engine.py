@@ -223,6 +223,48 @@ class Engine:
         greedy = torch.frombuffer(gr, dtype=torch.int32).clone()[:n - 1].to(torch.int64)
         return logprobs, greedy
 
+    def score_batch(self, seqs: Sequence[Sequence[int]],
+                    exit_layer: int = -1) -> List[Tuple[torch.Tensor, torch.Tensor]]:
+        """`score` of every sequence in `seqs`, in one call on the wgmma prompt pass: the rows of all
+        sequences share 128-token chunks, so short sequences no longer pay a whole weight pass each.
+        Returns one (logprobs float32[n-1], greedy int64[n-1]) per sequence, in order.  Each entry
+        is bit-identical to `score` of that sequence alone when it has more than max_rows + 1 ids
+        (shorter ones take the decode route in `score`).  Needs an engine with the prompt pass."""
+        seqs = [[int(t) for t in s] for s in seqs]
+        offsets = [0]
+        for s in seqs:
+            offsets.append(offsets[-1] + len(s))
+        flat = [t for s in seqs for t in s]
+        rows = offsets[-1] - len(seqs)
+        arr = (C.c_int32 * max(len(flat), 1))(*flat)
+        off = (C.c_int32 * len(offsets))(*offsets)
+        lp = (C.c_float * max(rows, 1))()
+        gr = (C.c_int32 * max(rows, 1))()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_score_batch(self._h, arr, off, len(seqs), int(exit_layer), lp, gr))
+        logprobs = torch.frombuffer(lp, dtype=torch.float32).clone()
+        greedy = torch.frombuffer(gr, dtype=torch.int32).clone().to(torch.int64)
+        out = []
+        for j, s in enumerate(seqs):
+            r0 = offsets[j] - j
+            out.append((logprobs[r0:r0 + len(s) - 1], greedy[r0:r0 + len(s) - 1]))
+        return out
+
+    def _loglikelihood_ids(self, context: Sequence[int], continuation: Sequence[int]) -> List[int]:
+        """The ids `loglikelihood` scores: validated, joined and truncated from the left."""
+        if not context or not continuation:
+            raise ValueError("context and continuation must both be non-empty")
+        if len(continuation) >= self.max_ctx:
+            raise ValueError(f"a continuation of {len(continuation)} tokens does not fit max_ctx "
+                             f"{self.max_ctx} with at least one context token")
+        return (list(context) + list(continuation))[-self.max_ctx:]
+
+    @staticmethod
+    def _continuation_score(logprobs: torch.Tensor, greedy: torch.Tensor,
+                            continuation: List[int]) -> Tuple[float, bool]:
+        k = len(continuation)
+        return float(logprobs[-k:].to(torch.float64).sum()), bool(greedy[-k:].tolist() == continuation)
+
     def loglikelihood(self, context: Sequence[int], continuation: Sequence[int],
                       exit_layer: int = -1) -> Tuple[float, bool]:
         """Log-likelihood of `continuation` following `context`, and whether greedy decoding from
@@ -234,17 +276,26 @@ class Engine:
         float64.  Both parts must be non-empty, and at least one token must precede the
         continuation after truncation (len(continuation) < max_ctx)."""
         context, continuation = [int(t) for t in context], [int(t) for t in continuation]
-        if not context or not continuation:
-            raise ValueError("context and continuation must both be non-empty")
-        if len(continuation) >= self.max_ctx:
-            raise ValueError(f"a continuation of {len(continuation)} tokens does not fit max_ctx "
-                             f"{self.max_ctx} with at least one context token")
-        ids = (context + continuation)[-self.max_ctx:]
-        logprobs, greedy = self.score(ids, exit_layer)
-        k = len(continuation)
-        total = float(logprobs[-k:].to(torch.float64).sum())
-        is_greedy = bool(greedy[-k:].tolist() == continuation)
-        return total, is_greedy
+        logprobs, greedy = self.score(self._loglikelihood_ids(context, continuation), exit_layer)
+        return self._continuation_score(logprobs, greedy, continuation)
+
+    def loglikelihood_batch(self, requests: Sequence[Tuple[Sequence[int], Sequence[int]]],
+                            exit_layer: int = -1) -> List[Tuple[float, bool]]:
+        """`loglikelihood` of every (context, continuation) request, in order, with one
+        `score_batch` call for all of them (every request is validated before any is scored).  On an
+        engine without the wgmma prompt pass it calls `loglikelihood` once per request.
+
+        Caveat: a request whose joined ids number at most max_rows + 1 is scored here on the wgmma
+        route, while `loglikelihood` scores it on the decode route.  The two then agree within the
+        oracle bounds, not bit for bit; longer requests agree bit for bit."""
+        reqs = [([int(t) for t in ctx], [int(t) for t in cont]) for ctx, cont in requests]
+        seqs = [self._loglikelihood_ids(ctx, cont) for ctx, cont in reqs]
+        if not reqs:
+            return []
+        if not (self.prefill_tc and self.arch.hidden % 64 == 0):
+            return [self.loglikelihood(ctx, cont, exit_layer) for ctx, cont in reqs]
+        scored = self.score_batch(seqs, exit_layer)
+        return [self._continuation_score(lp, gr, cont) for (lp, gr), (_, cont) in zip(scored, reqs)]
 
     # ------------------------------------------------------------------ introspection
     @property

@@ -19,12 +19,17 @@ SM_COUNT = 132                      # H100 SXM: one arg-max candidate slot per S
 
 def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling: bool = False,
                 keep_logits: bool = False, lm_head_tc: bool = False, prefill_tc: bool = True,
-                scoring: bool = False) -> Dict[str, int]:
+                scoring: bool = False, batch_scoring: bool = False) -> Dict[str, int]:
     """Bytes the engine allocates on ONE rank.  Keys: weights, embed, lm_head, kv_pool, scratch,
     total (+ weights_source_peak: the largest single tensor staged on the GPU while loading).
     `scoring` adds what the first `lsk_score` call allocates: the logits rows (unless already
-    there) and one float + one int per position."""
+    there) and one float + one int per position.  `batch_scoring` adds what the first
+    `lsk_score_batch` call allocates: the scoring buffers, eight ints per position (row ids,
+    targets, row map, attention pieces of a group) and one arrival counter per (piece, kv head)
+    of a 128-row chunk (nothing without the prompt pass, which refuses the call)."""
     h, L = arch.hidden, arch.layers
+    batch_scoring = batch_scoring and prefill_tc and h % 64 == 0
+    scoring = scoring or batch_scoring
     q_l = arch.heads // tp_size * arch.head_dim
     kv_l = arch.kv_heads // tp_size * arch.head_dim
     inter_l = arch.inter // tp_size
@@ -63,6 +68,8 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
         scratch += MAX_ROWS * vocab_l_pad * 4
     if scoring:
         scratch += 2 * max_pos * 4                          # per-position log-probabilities + arg-max ids
+    if batch_scoring:
+        scratch += 8 * max_pos * 4 + 128 * kvh_l * 4        # packed group arrays + piece arrival counters
     if sampling:
         scratch += (2 * MAX_ROWS + 1) * arch.vocab * 4
         if tp_size > 1:
