@@ -177,6 +177,24 @@ int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer,
 int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
                     int32_t exit_layer, float* logprob_out, int32_t* greedy_out);
 
+/* Teacher-forced scoring of ids[0..n-1] at n_exits exit layers in ONE pass, single GPU.  exits is
+ * strictly increasing, each in [1, n_layers], 1 <= n_exits <= LSK_MAX_EXITS.  Layers below each
+ * exit run once: the heads of the earlier exits run inside the pass of the deepest one.
+ *   logprob_out[j][i], greedy_out[j][i]  ([n_exits][n-1]; greedy may be NULL) are bit-identical to
+ *                                         lsk_score(ids, n, exits[j]) entry i
+ *   accept_out[j][i]  ([n_exits-1][n-1], may be NULL) = sum_v min(p_E(v), p_L(v)) for the row
+ *                     predicting ids[i+1]: p_E, p_L the warped (temperature, top-k, top-p)
+ *                     distributions at exit exits[j] and at full depth, i.e. the probability that
+ *                     the accept test of sampled self-speculation (self_speculation_generator.py:
+ *                     191-199) accepts a draft drawn at that exit.  It needs sampling->sample == 1,
+ *                     temperature > 0, no_repeat_ngram_size == 0 (the ban is not modelled) and
+ *                     exits[n_exits-1] == n_layers.  Only temperature, top_k and top_p are read.
+ * sampling may be NULL when accept_out is.  Same state rules as lsk_score. */
+#define LSK_MAX_EXITS 32
+int lsk_score_exits(lsk_engine* e, const int32_t* ids, int32_t n, const int32_t* exits, int32_t n_exits,
+                    const lsk_generation* sampling, float* logprob_out, int32_t* greedy_out,
+                    float* accept_out);
+
 /* Queries / debugging (parity tests). */
 int lsk_kv_len(const lsk_engine* e, int32_t* len_out);
 /* Teacher-forced block: the m given ids as one block at positions kv_len .. kv_len+m-1 through
@@ -267,6 +285,12 @@ int lsk_test_lmhead_tc(const void* w_bf16_dev, int64_t n, int64_t k, const float
  * logprob [rows] and the per-row arg-max greedy [rows] (nullable). */
 int lsk_test_logprob(const float* logits_dev, int32_t rows, int32_t vocab, int32_t ld,
                      const int32_t* targets_dev, float* logprob_dev, int32_t* greedy_dev);
+/* The acceptance kernels alone (csrc/sampling.cuh: warp_rows_kernel, accept_prob_kernel) on device
+ * buffers: draft and full-depth logits [rows][ld] fp32, the first `vocab` columns valid; writes
+ * accept_dev[r] = sum_v min of the two rows' warped distributions (temperature, top_k, top_p of
+ * `sampling`, temperature > 0). */
+int lsk_test_accept(const float* logits_draft_dev, const float* logits_verify_dev, int32_t rows,
+                    int32_t vocab, int32_t ld, const lsk_generation* sampling, float* accept_dev);
 
 #ifdef __cplusplus
 }

@@ -13,6 +13,7 @@ LIB_PATH = os.environ.get("LSK_LIB") or os.path.join(PKG_DIR, "liblsk.so")   # L
 
 LSK_MAX_SPEC = 15
 LSK_MAX_EOS = 8
+LSK_MAX_EXITS = 32
 LSK_FLAG_KEEP_LOGITS = 1
 LSK_FLAG_NO_PDL = 2
 LSK_FLAG_NO_GRAPH = 4
@@ -98,6 +99,9 @@ SIGNATURES = {
                             C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
     "lsk_score_batch": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
                                   C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
+    "lsk_score_exits": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32), C.c_int32,
+                                  C.POINTER(lsk_generation), C.POINTER(C.c_float), C.POINTER(C.c_int32),
+                                  C.POINTER(C.c_float)]),
     "lsk_kv_len": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "lsk_debug_forward_rows": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
     "lsk_debug_read": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64,
@@ -125,6 +129,8 @@ SIGNATURES = {
                                      C.c_int32, C.POINTER(C.c_float)]),
     "lsk_test_logprob": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                    C.c_void_p]),
+    "lsk_test_accept": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                  C.POINTER(lsk_generation), C.c_void_p]),
 }
 
 _lib = None

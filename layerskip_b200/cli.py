@@ -310,6 +310,94 @@ def main_score(argv=None):
     return results
 
 
+def predict_grid(eng, prompts: List[List[int]], exit_layers: List[int], num_speculations: List[int],
+                 gcfg: GenerationConfig, n_layers: int, seed: int = 0) -> List[Dict[str, Any]]:
+    """The sweep's (exit layer, num_speculations) grid predicted from one `score_exits` pass per
+    prompt (predict.py).  Each prompt is extended by max_steps tokens of full-depth generation: AR
+    greedy, or AR sampled with the generation config's warp, which has the distribution of sampled
+    self-speculation's output.  Greedy rows are exact; sampled rows use each exit's mean
+    acceptance probability in the i.i.d. formula and are marked exact = False."""
+    from . import predict
+    steps = gcfg.max_steps
+    exits = sorted(set(exit_layers) | {n_layers})
+    warp = {"temperature": gcfg.temperature, "top_k": gcfg.top_k, "top_p": gcfg.top_p} if gcfg.sample else None
+    g = torch.Generator().manual_seed(seed)
+    per_prompt: List[Dict[int, Any]] = []
+    for p in prompts:
+        eng.begin(-1, steps, [], sample=gcfg.sample, temperature=gcfg.temperature, top_k=gcfg.top_k,
+                  top_p=gcfg.top_p, seed=int(torch.randint(0, 2 ** 31 - 1, (), generator=g)))
+        eng.prefill(p)
+        cont = [eng.ar_step() for _ in range(steps)]
+        _lp, greedy, accept = eng.score_exits(p + cont, exits, warp)
+        rows = slice(len(p) - 1, len(p) - 1 + steps)      # row len(p) - 1 + q predicts cont[q]
+        want = torch.tensor(cont, dtype=torch.int64)
+        per = {}
+        for j, e in enumerate(exits):
+            if e not in exit_layers:
+                continue
+            if not warp:
+                per[e] = (greedy[j, rows] == want).tolist()
+            else:   # a draft at full depth is drawn from the verifier's own distribution: alpha = 1
+                per[e] = accept[j, rows] if e < n_layers else torch.ones(steps)
+        per_prompt.append(per)
+    out = []
+    for e in exit_layers:
+        if warp:
+            alpha = float(torch.cat([pp[e].to(torch.float64) for pp in per_prompt]).mean())
+        for d in num_speculations:
+            if warp:
+                acc, tpr = predict.sampled_estimate(alpha, d)
+                out.append({"exit_layer": e, "num_speculations": d, "acceptance_rate": acc,
+                            "tokens_per_round": tpr, "exact": False, "mean_alpha": alpha})
+            else:
+                rounds = [predict.greedy_rounds(pp[e], d, steps) for pp in per_prompt]
+                out.append({"exit_layer": e, "num_speculations": d,
+                            "acceptance_rate": predict.mean(predict.acceptance_rate(r) for r in rounds),
+                            "tokens_per_round": predict.mean(predict.tokens_per_round(r) for r in rounds),
+                            "exact": True})
+    return out
+
+
+def main_predict(argv=None):
+    """The sweep's grid (sweep.py:36-74 arguments) predicted from ONE teacher-forced pass per prompt
+    at every exit at once, instead of one benchmark per (E, D).  Writes predict_*.csv with
+    exit_layer, num_speculations, acceptance_rate, tokens_per_round, exact.  With --model_args
+    alpha=... the damping starts at exit_layer_first (as in `main_score`): the prediction is for
+    generations on that one model, not for `main_sweep`'s per-E models."""
+    if argv is not None:
+        sys.argv = [sys.argv[0]] + list(argv)
+    args, bargs, sargs, gcfg = parse(Arguments, BenchmarkArguments, SweepArguments, GenerationConfig)
+    if bargs.dataset != "synthetic":
+        raise NotImplementedError("only --dataset synthetic is available offline")
+    if gcfg.no_repeat_ngram_size:
+        raise NotImplementedError("the prediction does not model the n-gram ban (--no_repeat_ngram_size)")
+    exit_layers = list(range(sargs.exit_layer_first, sargs.exit_layer_last + 1, sargs.exit_layer_step))
+    specs = list(range(sargs.num_speculations_first, sargs.num_speculations_last + 1, sargs.num_speculations_step))
+    model, _tok, margs = load_model_and_tokenizer(args, sargs.exit_layer_first)
+    arch = model.arch
+    if not exit_layers or min(exit_layers) < 1 or max(exit_layers) > arch.layers:
+        raise ValueError(f"exit layers {exit_layers} must lie in [1, {arch.layers}]")
+    from .engine import Engine
+    max_ctx = max(int(margs.get("max_ctx", 0)), bargs.prompt_len + gcfg.max_steps + 2)
+    eng = Engine(arch, max_ctx=max_ctx)
+    try:
+        eng.load_model(model)
+        prompts = synthetic_prompts(arch.vocab, bargs.num_samples or 8, bargs.prompt_len)
+        rows = predict_grid(eng, prompts, exit_layers, specs, gcfg, arch.layers, args.seed or 0)
+    finally:
+        eng.close()
+    os.makedirs(args.output_dir, exist_ok=True)
+    path = os.path.join(args.output_dir, f"predict_{time.strftime('%Y%m%d_%H%M%S')}.csv")
+    fields = ["exit_layer", "num_speculations", "acceptance_rate", "tokens_per_round", "exact"]
+    with open(path, "w", newline="") as f:
+        wr = csv.DictWriter(f, fieldnames=fields, extrasaction="ignore")
+        wr.writeheader()
+        wr.writerows(rows)
+    for r in rows:
+        print({k: r[k] for k in fields + (["mean_alpha"] if "mean_alpha" in r else [])}, flush=True)
+    return rows
+
+
 class _PrintStreamer:
     """Plain-text stand-in for transformers.TextStreamer / SpeculativeTextStreamer."""
 

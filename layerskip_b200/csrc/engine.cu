@@ -13,6 +13,7 @@
 #include <cstring>
 #include <algorithm>
 #include <atomic>
+#include <functional>
 #include <map>
 #include <string>
 #include <vector>
@@ -155,6 +156,14 @@ struct lsk_engine {
   int* score_greedy = nullptr;         // lsk_score: [max_pos] arg-max ids
   int* batch_buf = nullptr;            // lsk_score_batch: [8][max_pos] row ids, targets, row map, pieces of a group
   unsigned int* piece_arrive = nullptr;  // lsk_score_batch: [128 pieces][kv heads] attention arrival counters
+  // lsk_score_exits (allocated on first use, grown with the number of exits)
+  int exits_cap = 0;                   // exits the result arrays hold
+  float* exits_lp = nullptr;           // [exits_cap][max_pos] log-probabilities
+  int* exits_greedy = nullptr;         // [exits_cap][max_pos] arg-max ids
+  int accept_cap = 0;                  // draft exits the acceptance buffers hold
+  float* exits_accept = nullptr;       // [accept_cap][max_pos] acceptance probabilities
+  float* exits_pd = nullptr;           // [accept_cap][128 or 16 rows][vocab] warped draft rows of the current chunk
+  float* exits_pv = nullptr;           // [16][vocab] warped full-depth rows of the current slice
   DevState* state = nullptr;
   GenParams* gen_dev = nullptr;
   RoundResult* res_host = nullptr;     // mapped pinned
@@ -640,13 +649,23 @@ struct PackedChunk {
   int n_pieces, max_piece_rows;
 };
 
+// Scoring at several exits in one pass (lsk_score_exits): at the top of layer layers[t] the first
+// norm kernel has folded the pending partials into hidden_p, exactly as the final fold of a pass
+// that stops there does, so head(t) reads the residual rows after layers [0, layers[t]).
+struct ChunkTaps {
+  const int* layers;             // strictly increasing, each in [1, n_run)
+  int n;
+  std::function<int(int)> head;
+};
+
 // Layers [0, n_run) run on the chunk.  The prompt pass (complete = false) stops the last of them
 // once its K/V rows are written; scoring (complete = true) runs it to the end and folds the pending
 // row-parallel partials into hidden_p, which then holds the residual rows the LM head reads.
 // With `pk` the rows are a packed chunk: ids, positions and pages come from it, and one piece-grid
-// attention launch per layer covers every piece (c0 is then unused).
+// attention launch per layer covers every piece (c0 is then unused).  With `taps` the heads of the
+// earlier exits run inside the pass.
 static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool complete,
-                                 const PackedChunk* pk = nullptr) {
+                                 const PackedChunk* pk = nullptr, const ChunkTaps* taps = nullptr) {
   const lsk_config& c = e->cfg;
   const bool tp = c.tp_size > 1;
   e->cur_class = CLS_MISC;
@@ -671,13 +690,14 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool c
     pend = e->tp_buf_p; n_pend = 1;
     return LSK_OK;
   };
-  for (int li = 0; li < n_run; ++li) {
+  for (int li = 0, tap = 0; li < n_run; ++li) {
     LayerWeights& L = e->layers[li];
     __nv_bfloat16* kp = e->kpool + (size_t)li * e->pool_layer_elems;
     __nv_bfloat16* vp = e->vpool + (size_t)li * e->pool_layer_elems;
     e->cur_class = CLS_QKV;
     CU(launch(e, rms_canon_kernel, dim3(m), dim3(256), 0, e->hidden_p, c.hidden, pend, n_pend, part_stride,
               (const __nv_bfloat16*)L.ln1, c.rms_eps, c.hidden, e->xn_c));
+    if (taps && tap < taps->n && taps->layers[tap] == li) TRY(taps->head(tap++));
     {
       PrefillGemmArgs a{};
       a.W = L.wqkv_c; a.X = e->xn_c; a.n_tiles = e->pf_t_qkv; a.n_rows = e->q_rows + 2 * e->kv_rows;
@@ -1240,7 +1260,8 @@ void lsk_destroy(lsk_engine* e) {
                   e->hidden, e->qbuf, e->attn_out, e->act, e->tp_buf, e->logits, e->logits_gath, e->logits_full, e->probs_d, e->probs_v, e->samp_scratch, e->cand_val,
                   e->cand_idx, e->gath_val, e->gath_idx, e->ban_val, e->ban_idx, e->rank_val, e->rank_idx,
                   e->d_zero, e->d_prompt, e->state, e->gen_dev, e->attn_part, e->attn_arrive,
-                  e->score_lp, e->score_greedy, e->batch_buf, e->piece_arrive};
+                  e->score_lp, e->score_greedy, e->batch_buf, e->piece_arrive, e->exits_lp, e->exits_greedy,
+                  e->exits_accept, e->exits_pd, e->exits_pv};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->res_host) cudaFreeHost(e->res_host);
   if (e->ev0) cudaEventDestroy(e->ev0);
@@ -1675,13 +1696,14 @@ static int alloc_scoring(lsk_engine* e, bool batch) {
 }
 
 // LM head + log softmax on M residual rows at x: the log-probabilities of targets[0 .. M) and the
-// arg-max ids go to score_lp / score_greedy from row r on.
-static int enqueue_score_head(lsk_engine* e, const float* x, int M, const int* targets, int r) {
+// arg-max ids go to lp / greedy (score_lp / score_greedy unless given) from row r on.
+static int enqueue_score_head(lsk_engine* e, const float* x, int M, const int* targets, int r,
+                              float* lp = nullptr, int* greedy = nullptr) {
   e->cur_class = CLS_LMHEAD;
   TRY(launch_lm_head_gemm(e, x, M, e->logits));
   e->cur_class = CLS_MISC;
   CU(launch(e, logprob_rows_kernel, dim3(M), dim3(kLogprobThreads), 0, (const float*)e->logits, e->vocab_l_pad,
-            e->vocab_l, targets, e->score_lp + r, e->score_greedy + r));
+            e->vocab_l, targets, (lp ? lp : e->score_lp) + r, (greedy ? greedy : e->score_greedy) + r));
   return LSK_OK;
 }
 
@@ -1827,6 +1849,136 @@ int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, i
     out_row += rows;
     j = k;
   }
+  CU(cudaStreamSynchronize(e->stream));
+  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
+  return LSK_OK;
+}
+
+// lsk_score_exits buffers: result rows for k exits, and with `accept` the acceptance rows and the
+// warped draft rows of k - 1 exits.  Allocated on first use; a call with more exits regrows them.
+static int alloc_score_exits(lsk_engine* e, int k, bool accept) {
+  auto realloc0 = [&](void** p, size_t bytes) -> int {
+    if (*p) cudaFree(*p);
+    *p = nullptr;
+    cudaError_t er = cudaMalloc(p, bytes);
+    if (er != cudaSuccess) {
+      *p = nullptr;
+      cudaGetLastError();
+      return fail(LSK_ERR_NOMEM, "lsk_score_exits: cudaMalloc of %zu bytes failed: %s", bytes, cudaGetErrorString(er));
+    }
+    return LSK_OK;
+  };
+  const size_t V = (size_t)e->cfg.vocab, P = (size_t)e->max_pos;
+  if (!e->logits) TRY(realloc0((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4));
+  if (k > e->exits_cap) {
+    e->exits_cap = 0;
+    TRY(realloc0((void**)&e->exits_lp, (size_t)k * P * 4));
+    TRY(realloc0((void**)&e->exits_greedy, (size_t)k * P * 4));
+    e->exits_cap = k;
+  }
+  if (accept && k - 1 > e->accept_cap) {
+    const size_t rows = e->pf_tc ? kPfTokens : kMaxRows;
+    e->accept_cap = 0;
+    TRY(realloc0((void**)&e->exits_accept, (size_t)(k - 1) * P * 4));
+    TRY(realloc0((void**)&e->exits_pd, (size_t)(k - 1) * rows * V * 4));
+    if (!e->exits_pv) TRY(realloc0((void**)&e->exits_pv, (size_t)kMaxRows * V * 4));
+    e->accept_cap = k - 1;
+  }
+  return LSK_OK;
+}
+
+// Teacher-forced scoring at several exits in one pass: the rows take lsk_score's route for the
+// deepest exit, and the head of every earlier exit runs where that exit's own pass would have
+// stopped (wgmma chunks: a tap at the top of layer E_j; decode blocks: after layer E_j - 1), so
+// every row is bit-identical to lsk_score at that exit.  With accept_out, each earlier exit's
+// head also warps its logits into the chunk's draft rows, and the full-depth head computes the
+// acceptance probability of every draft row against its own warped row.
+int lsk_score_exits(lsk_engine* e, const int32_t* ids, int32_t n, const int32_t* exits, int32_t n_exits,
+                    const lsk_generation* sampling, float* logprob_out, int32_t* greedy_out, float* accept_out) {
+  if (!e || !ids || !exits || !logprob_out) return fail(LSK_ERR_INVALID, "null argument");
+  if (accept_out && !sampling) return fail(LSK_ERR_INVALID, "accept_out needs the sampling settings (sampling is NULL)");
+  const lsk_config& c = e->cfg;
+  if (c.tp_size > 1)
+    return fail(LSK_ERR_INVALID, "lsk_score_exits needs tp_size 1: tensor-parallel scoring is not supported");
+  if (n < 2) return fail(LSK_ERR_INVALID, "scoring needs at least 2 ids (got %d)", n);
+  if (n > c.max_ctx) return fail(LSK_ERR_CTX, "sequence of %d ids exceeds max_ctx %d", n, c.max_ctx);
+  if (n_exits < 1 || n_exits > LSK_MAX_EXITS)
+    return fail(LSK_ERR_INVALID, "n_exits must be in [1, %d] (got %d)", LSK_MAX_EXITS, n_exits);
+  for (int j = 0; j < n_exits; ++j) {
+    if (exits[j] < 1 || exits[j] > c.n_layers)
+      return fail(LSK_ERR_INVALID, "exits[%d] = %d is outside [1, n_layers %d]", j, exits[j], c.n_layers);
+    if (j > 0 && exits[j] <= exits[j - 1])
+      return fail(LSK_ERR_INVALID, "exits must be strictly increasing (exits[%d] = %d, exits[%d] = %d)", j - 1,
+                  exits[j - 1], j, exits[j]);
+  }
+  for (int i = 0; i < n; ++i)
+    if (ids[i] < 0 || ids[i] >= c.vocab) return fail(LSK_ERR_INVALID, "token id %d out of range", ids[i]);
+  if (accept_out) {
+    if (sampling->sample != 1 || !(sampling->temperature > 0.f))
+      return fail(LSK_ERR_INVALID, "accept_out needs sampling settings with sample = 1 and temperature > 0");
+    if (sampling->no_repeat_ngram_size != 0)
+      return fail(LSK_ERR_INVALID, "accept_out does not model the n-gram ban: no_repeat_ngram_size must be 0");
+    if (exits[n_exits - 1] != c.n_layers)
+      return fail(LSK_ERR_INVALID, "accept_out needs the last exit at full depth (%d, got %d)", c.n_layers,
+                  exits[n_exits - 1]);
+  }
+  if (!lsk_weights_complete(e)) return fail(LSK_ERR_STATE, "weights not fully loaded");
+  TRY(alloc_score_exits(e, n_exits, accept_out != nullptr));
+  const int k = n_exits, E = exits[k - 1], rows = n - 1, V = c.vocab;
+  const bool tc = e->pf_tc && rows > e->max_rows;
+  const size_t P = (size_t)e->max_pos, pd_stride = (size_t)(tc ? kPfTokens : kMaxRows) * V;
+  const WarpParams wp = accept_out ? WarpParams{sampling->temperature, sampling->top_k, sampling->top_p}
+                                   : WarpParams{1.f, 0, 1.f};
+  e->prefilled = false;
+  e->host_len = 0;
+  // exit j's head on M residual rows at x: sequence rows r0 .., rows rc .. of the current chunk
+  auto head = [&](int j, const float* x, int r0, int rc, int M) -> int {
+    TRY(enqueue_score_head(e, x, M, e->d_prompt + r0 + 1, r0, e->exits_lp + j * P, e->exits_greedy + j * P));
+    if (!accept_out || k == 1) return LSK_OK;
+    e->cur_class = CLS_MISC;
+    if (j + 1 < k) {
+      CU(launch(e, warp_rows_kernel, dim3(M), dim3(kSampleThreads), 0, (const float*)e->logits, e->vocab_l_pad, V,
+                wp, e->exits_pd + j * pd_stride + (size_t)rc * V));
+    } else {
+      CU(launch(e, accept_prob_kernel, dim3(M), dim3(kSampleThreads), 0, (const float*)e->logits, e->vocab_l_pad, V,
+                wp, (const float*)(e->exits_pd + (size_t)rc * V), pd_stride, k - 1, e->exits_pv,
+                e->exits_accept + r0, P));
+    }
+    return LSK_OK;
+  };
+  CU(cudaEventRecord(e->ev0, e->stream));
+  CU(cudaMemcpyAsync(e->d_prompt, ids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  if (tc) {
+    for (int c0 = 0; c0 < rows; c0 += kPfTokens) {
+      const int m = std::min(rows - c0, kPfTokens);
+      auto slices = [&](int j) -> int {
+        for (int r0 = 0; r0 < m; r0 += e->max_rows)
+          TRY(head(j, e->hidden_p + (size_t)r0 * c.hidden, c0 + r0, r0, std::min(m - r0, e->max_rows)));
+        return LSK_OK;
+      };
+      const ChunkTaps taps{exits, k - 1, slices};
+      TRY(enqueue_prefill_chunk(e, c0, m, E, true, nullptr, k > 1 ? &taps : nullptr));
+      TRY(slices(k - 1));
+    }
+  } else {
+    for (int c0 = 0; c0 < rows; c0 += e->max_rows) {
+      const int m = std::min(rows - c0, e->max_rows);
+      TRY(emit_embed(e, e->d_prompt + c0, e->hidden, m));
+      for (int l = 0, j = 0; l < E; ++l) {
+        TRY(enqueue_layer(e, l, 0, m, e->d_zero, c0));
+        if (exits[j] == l + 1) TRY(head(j++, e->hidden, c0, 0, m));
+      }
+    }
+  }
+  CU(cudaEventRecord(e->ev1, e->stream));
+  CU(cudaMemcpy2DAsync(logprob_out, (size_t)rows * 4, e->exits_lp, P * 4, (size_t)rows * 4, k,
+                       cudaMemcpyDeviceToHost, e->stream));
+  if (greedy_out)
+    CU(cudaMemcpy2DAsync(greedy_out, (size_t)rows * 4, e->exits_greedy, P * 4, (size_t)rows * 4, k,
+                         cudaMemcpyDeviceToHost, e->stream));
+  if (accept_out && k > 1)
+    CU(cudaMemcpy2DAsync(accept_out, (size_t)rows * 4, e->exits_accept, P * 4, (size_t)rows * 4, k - 1,
+                         cudaMemcpyDeviceToHost, e->stream));
   CU(cudaStreamSynchronize(e->stream));
   CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
   return LSK_OK;
@@ -2237,6 +2389,27 @@ int lsk_test_logprob(const float* logits, int32_t rows, int32_t vocab, int32_t l
   logprob_rows_kernel<<<rows, kLogprobThreads>>>(logits, ld, vocab, (const int*)targets, logprob, (int*)greedy);
   CU(cudaGetLastError());
   CU(cudaDeviceSynchronize());
+  return LSK_OK;
+}
+
+// the acceptance kernels alone (unit test): draft and full-depth logits [rows][ld] fp32, the first
+// `vocab` columns valid; accept[r] = sum_v min of the two warped rows r
+int lsk_test_accept(const float* logits_draft, const float* logits_verify, int32_t rows, int32_t vocab, int32_t ld,
+                    const lsk_generation* sampling, float* accept) {
+  if (!logits_draft || !logits_verify || !sampling || !accept || rows < 1 || vocab < 1 || ld < vocab)
+    return fail(LSK_ERR_INVALID, "bad acceptance test shape");
+  if (!(sampling->temperature > 0.f)) return fail(LSK_ERR_INVALID, "acceptance test needs temperature > 0");
+  const WarpParams wp{sampling->temperature, sampling->top_k, sampling->top_p};
+  float* buf = nullptr;
+  CU(cudaMalloc((void**)&buf, (size_t)2 * rows * vocab * 4));
+  warp_rows_kernel<<<rows, kSampleThreads>>>(logits_draft, ld, vocab, wp, buf);
+  accept_prob_kernel<<<rows, kSampleThreads>>>(logits_verify, ld, vocab, wp, buf, (size_t)0, 1,
+                                               buf + (size_t)rows * vocab, accept, (size_t)0);
+  const cudaError_t er = cudaGetLastError();
+  const cudaError_t es = cudaDeviceSynchronize();
+  cudaFree(buf);
+  CU(er);
+  CU(es);
   return LSK_OK;
 }
 

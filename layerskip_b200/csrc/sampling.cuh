@@ -130,32 +130,22 @@ __device__ int block_sample_index(const float* __restrict__ w, int V, float u, f
   return *s_pick;
 }
 
-// One row per CTA: logits -> warped probabilities (written out) -> sampled token.
-//   grid.x rows; row r reads logits + r*ld, writes probs + r*V and tok_out[r].
-__global__ void __launch_bounds__(kSampleThreads)
-warp_and_sample_kernel(const float* __restrict__ logits, int ld, int V,
-                       const GenParams* __restrict__ gpp, const DevState* __restrict__ st,
-                       float* __restrict__ probs, int* __restrict__ tok_out, int purpose,
-                       int row_base) {
-  __shared__ float red[96 + 32];
-  __shared__ float hist[256];
-  __shared__ uint32_t s_prefix;
-  __shared__ float s_g;
-  __shared__ int s_pick;
-  pdl_launch_dependents();
-  pdl_wait();
-  const GenParams gp = *gpp;
-  const int row = blockIdx.x;
-  const float* lg = logits + (size_t)row * ld;
-  float* pr = probs + (size_t)row * V;
-  const float inv_t = 1.0f / gp.temperature;
+// The warp of decode_next_token on one logits row lg[0 .. V) by one CTA of kSampleThreads: logits
+// / T -> top-k threshold -> softmax -> nucleus -> renormalised probabilities in pr[0 .. V).  Shared
+// by the sampling path and the acceptance kernels below, so a predicted acceptance probability
+// uses the arithmetic generation draws from.  Ends with a barrier: pr is then readable by the
+// whole CTA.  Shared scratch: red [96 + 32], hist [256], s_prefix, s_g.
+__device__ __forceinline__ void warp_row(const float* __restrict__ lg, int V, float temperature, int top_k,
+                                         float top_p, float* __restrict__ pr, float* red, float* hist,
+                                         uint32_t& s_prefix, float& s_g) {
+  const float inv_t = 1.0f / temperature;
 
   // ---- top-k threshold (HF TopKLogitsWarper: drop scores < k-th largest)
   float kth = -INFINITY;
-  if (gp.top_k > 0 && gp.top_k < V) {
+  if (top_k > 0 && top_k < V) {
     __shared__ int cnt[256];
     uint32_t prefix = 0;
-    int need = gp.top_k;                 // how many keys >= threshold still to take
+    int need = top_k;                    // how many keys >= threshold still to take
     for (int level = 3; level >= 0; --level) {
       for (int i = threadIdx.x; i < 256; i += kSampleThreads) cnt[i] = 0;
       __syncthreads();
@@ -203,7 +193,7 @@ warp_and_sample_kernel(const float* __restrict__ logits, int ld, int V,
 
   // ---- nucleus: keep token i iff the mass of strictly larger tokens is < top_p
   uint32_t kstar = 0;                    // keep keys >= kstar
-  if (gp.top_p >= 0.f && gp.top_p < 1.0f) {
+  if (top_p >= 0.f && top_p < 1.0f) {
     uint32_t prefix = 0;
     float G = 0.f;                       // mass above the bucket being refined
     for (int level = 3; level >= 0; --level) {
@@ -221,7 +211,7 @@ warp_and_sample_kernel(const float* __restrict__ logits, int ld, int V,
         int b = 255;
         float g = G;
         for (; b > 0; --b) {
-          if (g + hist[b] >= gp.top_p) break;
+          if (g + hist[b] >= top_p) break;
           g += hist[b];
         }
         s_g = g;
@@ -251,11 +241,82 @@ warp_and_sample_kernel(const float* __restrict__ logits, int ld, int V,
     pr[j] = keep ? e * inv_z2 : 0.f;
   }
   __syncthreads();
+}
+
+// One row per CTA: logits -> warped probabilities (written out) -> sampled token.
+//   grid.x rows; row r reads logits + r*ld, writes probs + r*V and tok_out[r].
+__global__ void __launch_bounds__(kSampleThreads)
+warp_and_sample_kernel(const float* __restrict__ logits, int ld, int V,
+                       const GenParams* __restrict__ gpp, const DevState* __restrict__ st,
+                       float* __restrict__ probs, int* __restrict__ tok_out, int purpose,
+                       int row_base) {
+  __shared__ float red[96 + 32];
+  __shared__ float hist[256];
+  __shared__ uint32_t s_prefix;
+  __shared__ float s_g;
+  __shared__ int s_pick;
+  pdl_launch_dependents();
+  pdl_wait();
+  const GenParams gp = *gpp;
+  const int row = blockIdx.x;
+  float* pr = probs + (size_t)row * V;
+  warp_row(logits + (size_t)row * ld, V, gp.temperature, gp.top_k, gp.top_p, pr, red, hist, s_prefix, s_g);
 
   // ---- multinomial draw
   const float u = rng_uniform(gp, st->step_count, row_base + row, purpose);
   const int tok = block_sample_index(pr, V, u, red, &s_pick);
   if (threadIdx.x == 0) tok_out[row] = tok;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Acceptance probability of a sampled draft (lsk_score_exits).  The accept test u < min(1, p_L(t)
+// / p_E(t)) with t ~ p_E accepts with probability alpha = sum_v min(p_E(v), p_L(v)), p the warped
+// distributions of one position at the exit E and at full depth.  The warp settings travel by
+// value: a scoring call never touches a generation's GenParams.
+// ---------------------------------------------------------------------------------------------
+struct WarpParams {
+  float temperature;
+  int top_k;
+  float top_p;
+};
+
+// grid.x rows: row r of logits (ld floats apart, V valid columns) -> warped row at probs + r*V
+__global__ void __launch_bounds__(kSampleThreads)
+warp_rows_kernel(const float* __restrict__ logits, int ld, int V, WarpParams wp, float* __restrict__ probs) {
+  __shared__ float red[96 + 32];
+  __shared__ float hist[256];
+  __shared__ uint32_t s_prefix;
+  __shared__ float s_g;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int row = blockIdx.x;
+  warp_row(logits + (size_t)row * ld, V, wp.temperature, wp.top_k, wp.top_p, probs + (size_t)row * V, red, hist,
+           s_prefix, s_g);
+}
+
+// grid.x full-depth rows: warp row r of logits into scratch + r*V, then for every draft exit j
+// accept[j * accept_ld + r] = sum_v min(p_draft[j * draft_stride + r*V + v], p_full(v)): per-thread
+// strided sums merged by block_sum, a fixed order, so the result is bit-reproducible.
+__global__ void __launch_bounds__(kSampleThreads)
+accept_prob_kernel(const float* __restrict__ logits, int ld, int V, WarpParams wp,
+                   const float* __restrict__ p_draft, size_t draft_stride, int n_draft,
+                   float* __restrict__ scratch, float* __restrict__ accept, size_t accept_ld) {
+  __shared__ float red[96 + 32];
+  __shared__ float hist[256];
+  __shared__ uint32_t s_prefix;
+  __shared__ float s_g;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int row = blockIdx.x;
+  float* pv = scratch + (size_t)row * V;
+  warp_row(logits + (size_t)row * ld, V, wp.temperature, wp.top_k, wp.top_p, pv, red, hist, s_prefix, s_g);
+  for (int j = 0; j < n_draft; ++j) {
+    const float* pd = p_draft + j * draft_stride + (size_t)row * V;
+    float s = 0.f;
+    for (int v = threadIdx.x; v < V; v += kSampleThreads) s += fminf(pd[v], pv[v]);
+    s = block_sum(s, red);
+    if (threadIdx.x == 0) accept[j * accept_ld + row] = s;
+  }
 }
 
 // Rejection test + commit for the sampling path (self_speculation_generator.py:191-221).

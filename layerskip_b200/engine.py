@@ -250,6 +250,39 @@ class Engine:
             out.append((logprobs[r0:r0 + len(s) - 1], greedy[r0:r0 + len(s) - 1]))
         return out
 
+    def score_exits(self, ids: Sequence[int], exits: Sequence[int], sampling: Optional[Dict] = None
+                    ) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
+        """`score(ids, E)` at every exit E of `exits` (strictly increasing, in [1, layers]) in one
+        pass: layers below each exit run once.  Returns (logprobs float32[k, n-1], greedy
+        int64[k, n-1], accept): row j is bit-identical to `score(ids, exits[j])`.
+
+        With `sampling` (a dict with `temperature`, `top_k`, `top_p`), `exits[-1]` must be the full
+        depth, and accept float32[k-1, n-1] holds, for the row predicting ids[i+1], the probability
+        sum_v min(p_E(v), p_full(v)) that sampled self-speculation accepts a draft drawn at exit
+        exits[j]: p are the warped distributions generation draws from.  accept is None without
+        `sampling`.  Ends any generation in progress, like `score`."""
+        n, k = len(ids), len(exits)
+        arr = (C.c_int32 * max(n, 1))(*[int(t) for t in ids])
+        ex = (C.c_int32 * max(k, 1))(*[int(e) for e in exits])
+        rows = max(n - 1, 1)
+        lp = (C.c_float * (max(k, 1) * rows))()
+        gr = (C.c_int32 * (max(k, 1) * rows))()
+        gen, acc = None, None
+        if sampling is not None:
+            gen = _lib.lsk_generation(sample=1, temperature=float(sampling.get("temperature", 1.0)),
+                                      top_k=int(sampling.get("top_k", 0) or 0),
+                                      top_p=float(sampling.get("top_p", 1.0)))
+            acc = (C.c_float * (max(k - 1, 1) * rows))()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_score_exits(self._h, arr, n, ex, k, C.byref(gen) if gen is not None else None,
+                                                 lp, gr, acc))
+        logprobs = torch.frombuffer(lp, dtype=torch.float32).clone()[:k * (n - 1)].view(k, n - 1)
+        greedy = torch.frombuffer(gr, dtype=torch.int32).clone()[:k * (n - 1)].view(k, n - 1).to(torch.int64)
+        accept = None
+        if acc is not None:
+            accept = torch.frombuffer(acc, dtype=torch.float32).clone()[:(k - 1) * (n - 1)].view(k - 1, n - 1)
+        return logprobs, greedy, accept
+
     def _loglikelihood_ids(self, context: Sequence[int], continuation: Sequence[int]) -> List[int]:
         """The ids `loglikelihood` scores: validated, joined and truncated from the left."""
         if not context or not continuation:
