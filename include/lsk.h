@@ -291,6 +291,32 @@ int lsk_test_logprob(const float* logits_dev, int32_t rows, int32_t vocab, int32
  * `sampling`, temperature > 0). */
 int lsk_test_accept(const float* logits_draft_dev, const float* logits_verify_dev, int32_t rows,
                     int32_t vocab, int32_t ld, const lsk_generation* sampling, float* accept_dev);
+/* The sampling kernels alone (csrc/sampling.cuh).  `_dev` pointers are device pointers, the others
+ * host pointers.  Of `sampling` the draw reads temperature (> 0), top_k, top_p and seed, the accept
+ * test seed, n_eos and eos_ids.  The random number of a draw is Philox4x32-10 at counter (step
+ * count, row, purpose, 0x4c534b) under key (seed low, seed high): u = (first word >> 8) * 2^-24;
+ * purposes: 1 draft draw, 2 verifier draw, 3 accept test, 4 residual draw.
+ *
+ * lsk_test_draw: the inverse-CDF draw (block_sample_index) over weights_dev[vocab] (fp32, >= 0, any
+ * total), once per u_dev[i] in [0, 1): picks_dev[i] = the token whose interval of the running sum
+ * holds u * total; 0 for an all-zero row. */
+int lsk_test_draw(const float* weights_dev, int32_t vocab, const float* u_dev, int32_t n, int32_t* picks_dev);
+/* lsk_test_sample: warp_and_sample_kernel, the kernel generation draws with, on logits_dev [rows][ld]
+ * (the first `vocab` columns valid), n_steps times with step counts step0 .. step0 + n_steps - 1:
+ * row r draws at counter row row_base + r.  probs_dev [rows][vocab] receives the warped rows (of the
+ * first step; they do not depend on the step), tokens_dev [n_steps][rows] the drawn tokens. */
+int lsk_test_sample(const float* logits_dev, int32_t rows, int32_t vocab, int32_t ld,
+                    const lsk_generation* sampling, int32_t step0, int32_t n_steps, int32_t purpose,
+                    int32_t row_base, float* probs_dev, int32_t* tokens_dev);
+/* lsk_test_accept_sample: accept_sample_kernel (rejection test, residual resample, commit) on warped
+ * rows p_draft_dev [d][vocab] and p_verify_dev [d + 1][vocab], 1 <= d <= LSK_MAX_SPEC, n_steps times.
+ * Step s starts from a fresh state (committed length kv_len0, step count step0 + s) holding the draft
+ * tokens draft_ids [s][d] and the verifier's draws verified_ids [s][d + 1], and fills out[s];
+ * residual_dev [vocab] is the kernel's residual scratch, left as the last rejecting step wrote it. */
+int lsk_test_accept_sample(const float* p_draft_dev, const float* p_verify_dev, int32_t vocab, int32_t d,
+                           const int32_t* draft_ids, const int32_t* verified_ids,
+                           const lsk_generation* sampling, int32_t kv_len0, int32_t step0, int32_t n_steps,
+                           lsk_round_out* out, float* residual_dev);
 
 #ifdef __cplusplus
 }

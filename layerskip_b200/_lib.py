@@ -131,6 +131,12 @@ SIGNATURES = {
                                    C.c_void_p]),
     "lsk_test_accept": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                   C.POINTER(lsk_generation), C.c_void_p]),
+    "lsk_test_draw": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
+    "lsk_test_sample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(lsk_generation),
+                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "lsk_test_accept_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
+                                         C.POINTER(C.c_int32), C.POINTER(lsk_generation), C.c_int32, C.c_int32,
+                                         C.c_int32, C.POINTER(lsk_round_out), C.c_void_p]),
 }
 
 _lib = None

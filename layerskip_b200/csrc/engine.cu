@@ -2414,3 +2414,122 @@ int lsk_test_accept(const float* logits_draft, const float* logits_verify, int32
 }
 
 }  // extern "C"
+
+// device buffers of one stand-alone sampling test call, released when it returns
+struct TestBuffers {
+  std::vector<void*> ptrs;
+  ~TestBuffers() {
+    for (void* p : ptrs) cudaFree(p);
+  }
+  template <typename T>
+  cudaError_t alloc(T** out, size_t count) {
+    const cudaError_t er = cudaMalloc((void**)out, std::max<size_t>(count, 1) * sizeof(T));
+    if (er == cudaSuccess) ptrs.push_back(*out);
+    return er;
+  }
+};
+
+static GenParams gen_params_of(const lsk_generation& g) {
+  GenParams gp{};
+  gp.n_eos = g.n_eos;
+  for (int i = 0; i < g.n_eos; ++i) gp.eos[i] = g.eos_ids[i];
+  gp.sample = 1;
+  gp.temperature = g.temperature;
+  gp.top_k = g.top_k;
+  gp.top_p = g.top_p;
+  gp.seed = g.seed;
+  return gp;
+}
+
+extern "C" {
+
+// the inverse-CDF draw alone (unit test): one CTA per u
+int lsk_test_draw(const float* weights, int32_t vocab, const float* u, int32_t n, int32_t* picks) {
+  if (!weights || !u || !picks || vocab < 1 || n < 1) return fail(LSK_ERR_INVALID, "bad draw test shape");
+  draw_index_kernel<<<n, kSampleThreads>>>(weights, vocab, u, (int*)picks);
+  CU(cudaGetLastError());
+  CU(cudaDeviceSynchronize());
+  return LSK_OK;
+}
+
+// the generation sampling kernel alone (unit test): step s of n_steps runs with step_count = step0 + s
+int lsk_test_sample(const float* logits, int32_t rows, int32_t vocab, int32_t ld, const lsk_generation* sampling,
+                    int32_t step0, int32_t n_steps, int32_t purpose, int32_t row_base, float* probs,
+                    int32_t* tokens) {
+  if (!logits || !sampling || !probs || !tokens || rows < 1 || vocab < 1 || ld < vocab || n_steps < 1 || step0 < 0)
+    return fail(LSK_ERR_INVALID, "bad sampling test shape");
+  if (!(sampling->temperature > 0.f)) return fail(LSK_ERR_INVALID, "sampling test needs temperature > 0");
+  const GenParams gp = gen_params_of(*sampling);
+  std::vector<DevState> states((size_t)n_steps);
+  for (int s = 0; s < n_steps; ++s) {
+    states[s] = DevState{};
+    states[s].step_count = step0 + s;
+  }
+  TestBuffers bufs;
+  GenParams* gp_dev = nullptr;
+  DevState* st_dev = nullptr;
+  float* later = nullptr;                // the warped rows of steps > 0 (the same values again)
+  CU(bufs.alloc(&gp_dev, 1));
+  CU(bufs.alloc(&st_dev, (size_t)n_steps));
+  if (n_steps > 1) CU(bufs.alloc(&later, (size_t)rows * vocab));
+  CU(cudaMemcpy(gp_dev, &gp, sizeof(gp), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(st_dev, states.data(), states.size() * sizeof(DevState), cudaMemcpyHostToDevice));
+  for (int s = 0; s < n_steps; ++s)
+    warp_and_sample_kernel<<<rows, kSampleThreads>>>(logits, ld, vocab, gp_dev, st_dev + s, s == 0 ? probs : later,
+                                                     (int*)tokens + (size_t)s * rows, purpose, row_base);
+  CU(cudaGetLastError());
+  CU(cudaDeviceSynchronize());
+  return LSK_OK;
+}
+
+// the sampled accept / resample kernel alone (unit test): every step starts from a fresh state
+int lsk_test_accept_sample(const float* p_draft, const float* p_verify, int32_t vocab, int32_t d,
+                           const int32_t* draft_ids, const int32_t* verified_ids, const lsk_generation* sampling,
+                           int32_t kv_len0, int32_t step0, int32_t n_steps, lsk_round_out* out, float* residual) {
+  if (!p_draft || !p_verify || !draft_ids || !verified_ids || !sampling || !out || !residual || vocab < 1 ||
+      d < 1 || d > LSK_MAX_SPEC || n_steps < 1 || step0 < 0 || kv_len0 < 0 || sampling->n_eos < 0 ||
+      sampling->n_eos > LSK_MAX_EOS)
+    return fail(LSK_ERR_INVALID, "bad accept-sample test shape");
+  for (size_t i = 0; i < (size_t)n_steps * d; ++i)
+    if (draft_ids[i] < 0 || draft_ids[i] >= vocab) return fail(LSK_ERR_INVALID, "draft id outside the vocabulary");
+  const GenParams gp = gen_params_of(*sampling);
+  std::vector<DevState> states((size_t)n_steps);
+  for (int s = 0; s < n_steps; ++s) {
+    DevState& st = states[s];
+    st = DevState{};
+    st.len = kv_len0;
+    st.step_count = step0 + s;
+    for (int i = 0; i < d; ++i) st.tok[1 + i] = draft_ids[(size_t)s * d + i];
+    for (int i = 0; i <= d; ++i) st.verified[i] = verified_ids[(size_t)s * (d + 1) + i];
+  }
+  TestBuffers bufs;
+  GenParams* gp_dev = nullptr;
+  DevState* st_dev = nullptr;
+  RoundResult* res_dev = nullptr;
+  CU(bufs.alloc(&gp_dev, 1));
+  CU(bufs.alloc(&st_dev, (size_t)n_steps));
+  CU(bufs.alloc(&res_dev, (size_t)n_steps));
+  CU(cudaMemcpy(gp_dev, &gp, sizeof(gp), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(st_dev, states.data(), states.size() * sizeof(DevState), cudaMemcpyHostToDevice));
+  CU(cudaMemset(res_dev, 0, (size_t)n_steps * sizeof(RoundResult)));
+  for (int s = 0; s < n_steps; ++s)
+    accept_sample_kernel<<<1, kSampleThreads>>>(p_draft, p_verify, vocab, d, st_dev + s, gp_dev, res_dev + s,
+                                                residual, s + 1, (int*)nullptr);
+  CU(cudaGetLastError());
+  CU(cudaDeviceSynchronize());
+  std::vector<RoundResult> res((size_t)n_steps);
+  CU(cudaMemcpy(res.data(), res_dev, res.size() * sizeof(RoundResult), cudaMemcpyDeviceToHost));
+  for (int s = 0; s < n_steps; ++s) {
+    const RoundResult& r = res[s];
+    lsk_round_out& o = out[s];
+    o.n_drafted = r.n_drafted; o.n_matches = r.n_matches; o.n_emitted = r.n_emitted; o.kv_len = r.kv_len;
+    for (int i = 0; i <= LSK_MAX_SPEC; ++i) {
+      o.draft_ids[i] = r.draft_ids[i];
+      o.emitted_ids[i] = r.emitted_ids[i];
+      o.verified_ids[i] = r.verified_ids[i];
+    }
+  }
+  return LSK_OK;
+}
+
+}  // extern "C"

@@ -73,8 +73,14 @@ __device__ __forceinline__ uint32_t fkey(float f) {
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
-// Inverse-CDF draw over weights w[0..V) in index order (torch.multinomial's distribution):
-// returns the smallest j with sum_{i<=j} w_i > target * total.  Contiguous chunk per thread.
+// Inverse-CDF draw over weights w[0..V) in index order (torch.multinomial's distribution): the
+// token whose interval of the running sum holds target = u * total.  Contiguous chunk per thread;
+// before_t is the fp32 block scan of the chunk sums.  In fp32 before_t + local_t is not
+// before_{t+1}, so intervals [before_t, before_t + local_t) would leave gaps and overlaps of a few
+// ulps at thread boundaries.  Instead the LAST thread with a positive chunk sum and before_t <=
+// target owns the target (a max over thread ids: one owner, whatever the order), and walks its own
+// chunk: the first token whose running sum exceeds target, else the chunk's last positive weight.
+// An all-zero row has no owner: token 0.
 __device__ int block_sample_index(const float* __restrict__ w, int V, float u, float* red,
                                   int* s_pick) {
   const int chunk = (V + kSampleThreads - 1) / kSampleThreads;
@@ -103,40 +109,54 @@ __device__ int block_sample_index(const float* __restrict__ w, int V, float u, f
     red[64 + l] = ti - t;              // exclusive prefix of warp totals
     if (l == 31) red[32] = ti;         // grand total
   }
-  if (threadIdx.x == 0) *s_pick = -1;
+  if (threadIdx.x == 0) *s_pick = -1;  // holds the owning thread first, then its pick
   __syncthreads();
   const float total = red[32];
   const float target = u * total;
   const float before = red[64 + wp] + (incl - local);
-  if (local > 0.f && target >= before && target < before + local) {
+  if (local > 0.f && target >= before) atomicMax(s_pick, (int)threadIdx.x);
+  __syncthreads();
+  const int owner = *s_pick;
+  __syncthreads();
+  if (owner < 0) return 0;
+  if ((int)threadIdx.x == owner) {
     float run = before;
-    int pick = hi - 1;
+    int pick = lo;
     for (int j = lo; j < hi; ++j) {
-      run += w[j];
-      if (target < run) { pick = j; break; }
+      const float wj = w[j];
+      if (wj > 0.f) {
+        pick = j;
+        run += wj;
+        if (target < run) break;
+      }
     }
     *s_pick = pick;
   }
   __syncthreads();
-  if (*s_pick < 0) {                    // rounding at the very end of the CDF: last positive weight
-    if (threadIdx.x == 0) {
-      int pick = 0;
-      for (int j = V - 1; j >= 0; --j)
-        if (w[j] > 0.f) { pick = j; break; }
-      *s_pick = pick;
-    }
-    __syncthreads();
-  }
   return *s_pick;
+}
+
+// block_sample_index alone (lsk_test_draw): CTA i draws from w[0..V) at u[i].
+__global__ void __launch_bounds__(kSampleThreads)
+draw_index_kernel(const float* __restrict__ w, int V, const float* __restrict__ u, int* __restrict__ picks) {
+  __shared__ float red[96 + 32];
+  __shared__ int s_pick;
+  const int pick = block_sample_index(w, V, u[blockIdx.x], red, &s_pick);
+  if (threadIdx.x == 0) picks[blockIdx.x] = pick;
 }
 
 // The warp of decode_next_token on one logits row lg[0 .. V) by one CTA of kSampleThreads: logits
 // / T -> top-k threshold -> softmax -> nucleus -> renormalised probabilities in pr[0 .. V).  Shared
 // by the sampling path and the acceptance kernels below, so a predicted acceptance probability
 // uses the arithmetic generation draws from.  Ends with a barrier: pr is then readable by the
-// whole CTA.  Shared scratch: red [96 + 32], hist [256], s_prefix, s_g.
+// whole CTA.  Shared scratch: red [96 + 32], hist [512], s_prefix, s_g.
+// The nucleus masses are summed as integers (probability * 2^43, truncated; two 32-bit limbs per
+// bucket, hist[b] the high and hist[256 + b] the low 12 bits, neither of which can overflow below a
+// vocabulary of 2^20): the atomic bucket sums then do not depend on the order the threads arrive in,
+// so a row whose mass sits on top_p keeps the same support every time.
+constexpr float kMassScale = 8796093022208.f;   // 2^43
 __device__ __forceinline__ void warp_row(const float* __restrict__ lg, int V, float temperature, int top_k,
-                                         float top_p, float* __restrict__ pr, float* red, float* hist,
+                                         float top_p, float* __restrict__ pr, float* red, uint32_t* hist,
                                          uint32_t& s_prefix, float& s_g) {
   const float inv_t = 1.0f / temperature;
 
@@ -194,32 +214,40 @@ __device__ __forceinline__ void warp_row(const float* __restrict__ lg, int V, fl
   // ---- nucleus: keep token i iff the mass of strictly larger tokens is < top_p
   uint32_t kstar = 0;                    // keep keys >= kstar
   if (top_p >= 0.f && top_p < 1.0f) {
+    __shared__ unsigned long long s_mass;
+    const unsigned long long p_fix = (unsigned long long)((double)top_p * (double)kMassScale);
     uint32_t prefix = 0;
-    float G = 0.f;                       // mass above the bucket being refined
+    unsigned long long G = 0;            // mass above the bucket being refined
     for (int level = 3; level >= 0; --level) {
-      for (int i = threadIdx.x; i < 256; i += kSampleThreads) hist[i] = 0.f;
+      for (int i = threadIdx.x; i < 512; i += kSampleThreads) hist[i] = 0u;
       __syncthreads();
       const uint32_t hi_mask = level == 3 ? 0u : (0xffffffffu << (8 * (level + 1)));
       for (int j = threadIdx.x; j < V; j += kSampleThreads) {
         const float p = pr[j] * inv_z;
         const uint32_t k = __float_as_uint(p);       // p >= 0: bit order == value order
         if (p > 0.f && (k & hi_mask) == (prefix & hi_mask))
-          atomicAdd(&hist[(k >> (8 * level)) & 255], p);
+        {
+          const unsigned long long q = __float2ull_rz(p * kMassScale);
+          const int b = (k >> (8 * level)) & 255;
+          atomicAdd(&hist[b], (uint32_t)(q >> 12));
+          atomicAdd(&hist[256 + b], (uint32_t)q & 4095u);
+        }
       }
       __syncthreads();
       if (threadIdx.x == 0) {
         int b = 255;
-        float g = G;
+        unsigned long long g = G;
         for (; b > 0; --b) {
-          if (g + hist[b] >= top_p) break;
-          g += hist[b];
+          const unsigned long long h = ((unsigned long long)hist[b] << 12) + hist[256 + b];
+          if (g + h >= p_fix) break;
+          g += h;
         }
-        s_g = g;
+        s_mass = g;
         s_prefix = prefix | ((uint32_t)b << (8 * level));
       }
       __syncthreads();
       prefix = s_prefix;
-      G = s_g;
+      G = s_mass;
     }
     kstar = prefix;
   }
@@ -251,7 +279,7 @@ warp_and_sample_kernel(const float* __restrict__ logits, int ld, int V,
                        float* __restrict__ probs, int* __restrict__ tok_out, int purpose,
                        int row_base) {
   __shared__ float red[96 + 32];
-  __shared__ float hist[256];
+  __shared__ uint32_t hist[512];
   __shared__ uint32_t s_prefix;
   __shared__ float s_g;
   __shared__ int s_pick;
@@ -284,7 +312,7 @@ struct WarpParams {
 __global__ void __launch_bounds__(kSampleThreads)
 warp_rows_kernel(const float* __restrict__ logits, int ld, int V, WarpParams wp, float* __restrict__ probs) {
   __shared__ float red[96 + 32];
-  __shared__ float hist[256];
+  __shared__ uint32_t hist[512];
   __shared__ uint32_t s_prefix;
   __shared__ float s_g;
   pdl_launch_dependents();
@@ -302,7 +330,7 @@ accept_prob_kernel(const float* __restrict__ logits, int ld, int V, WarpParams w
                    const float* __restrict__ p_draft, size_t draft_stride, int n_draft,
                    float* __restrict__ scratch, float* __restrict__ accept, size_t accept_ld) {
   __shared__ float red[96 + 32];
-  __shared__ float hist[256];
+  __shared__ uint32_t hist[512];
   __shared__ uint32_t s_prefix;
   __shared__ float s_g;
   pdl_launch_dependents();
