@@ -96,7 +96,6 @@ struct lsk_engine {
   int heads_l = 0, kv_heads_l = 0, q_rows = 0, kv_rows = 0, inter_l = 0, vocab_l = 0,
       vocab_l_pad = 0, vocab_off = 0, group = 0, inter_l_pad = 0;
   int n_pages = 0, max_pos = 0, n_splits = 0;
-  int attn_stages = 4;                 // K/V ring depth of the attention kernel (LSK_ATTN_STAGES, 2..4)
   int max_rows = kMaxRows;             // token rows one step can carry (8 when 16 do not fit)
   bool use_pdl = true, use_graph = true, keep_logits = false;
 
@@ -170,7 +169,6 @@ struct lsk_engine {
   RoundResult* res_dev = nullptr;      // device alias of res_host
 
   GemmPlan p_qkv, p_o, p_gu, p_d, p_lm;
-  size_t l2_prefetch_bytes = 0;          // LSK_L2_PREFETCH_MB: head of the NEXT kernel's weights pulled into L2 (A/B: no gain, +11 % traffic -> off)
   int lm_cand = 0;                     // candidates produced by the wgmma LM head (its grid)
   const float* cur_cand_val = nullptr;  // candidates of the last enqueued LM head (epilogue's, or the banned rows' arg-max)
   const int* cur_cand_idx = nullptr;
@@ -192,7 +190,6 @@ struct lsk_engine {
   lsk_generation gen{};
   bool began = false, prefilled = false;
   int host_len = 0;                    // host mirror of the committed KV length
-  int seq = 0;
   int64_t launches = 0;
   int64_t capture_launches = 0;        // launches recorded while capturing the current graph
   std::map<long long, int64_t> graph_launches;
@@ -208,8 +205,27 @@ enum { CLS_QKV = 0, CLS_ATTN = 1, CLS_O = 2, CLS_GATEUP = 3, CLS_DOWN = 4, CLS_L
 static constexpr int kSmemMax = 227 * 1024;
 
 // ---------------------------------------------------------------------------------------------
-// launch helper (programmatic dependent launch attribute on every kernel)
+// launch helpers
 // ---------------------------------------------------------------------------------------------
+// One piece of work enqueued on the engine's stream: counted as one launch and, when profiling,
+// timed by an event pair under kernel class `cls`.  Every kernel goes through it by way of
+// launch(); the NCCL all-reduces call it directly.
+template <typename F>
+static auto stream_op(lsk_engine* e, int cls, F enqueue) -> decltype(enqueue()) {
+  e->launches += 1;
+  e->capture_launches += 1;
+  if (!e->profiling) return enqueue();
+  cudaEvent_t a, b;
+  cudaEventCreate(&a);
+  cudaEventCreate(&b);
+  cudaEventRecord(a, e->stream);
+  auto err = enqueue();
+  cudaEventRecord(b, e->stream);
+  e->prof_events.push_back({cls, {a, b}});
+  return err;
+}
+
+// Kernel launch: programmatic dependent launch attribute on every kernel, class = e->cur_class.
 template <typename... KArgs, typename... Args>
 static cudaError_t launch(lsk_engine* e, void (*kern)(KArgs...), dim3 grid, dim3 block,
                           size_t smem, Args... args) {
@@ -223,28 +239,33 @@ static cudaError_t launch(lsk_engine* e, void (*kern)(KArgs...), dim3 grid, dim3
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
   cfg.numAttrs = e->use_pdl ? 1 : 0;
-  e->launches += 1;
-  e->capture_launches += 1;
-  if (!e->profiling) return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
-  cudaEvent_t a, b;
-  cudaEventCreate(&a);
-  cudaEventCreate(&b);
-  cudaEventRecord(a, e->stream);
-  cudaError_t err = cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
-  cudaEventRecord(b, e->stream);
-  e->prof_events.push_back({e->cur_class, {a, b}});
+  return stream_op(e, e->cur_class, [&]() { return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...); });
+}
+
+// Opt kernel `Kern` in to kSmemMax of dynamic shared memory, once per device (the attribute is per
+// DEVICE: one process may drive engines on several GPUs).  Done lazily at the launch site: the
+// stand-alone test entry points launch through an engine that lsk_create never set up.
+template <auto Kern>
+static cudaError_t allow_max_smem() {
+  static std::atomic<uint64_t> configured{0};
+  int dev = 0;
+  cudaError_t err = cudaGetDevice(&dev);
+  if (err != cudaSuccess) return err;
+  const uint64_t bit = 1ull << (dev & 63);
+  if (configured.load(std::memory_order_relaxed) & bit) return cudaSuccess;
+  err = cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax);
+  if (err == cudaSuccess) configured.fetch_or(bit, std::memory_order_relaxed);
   return err;
 }
 
 // ---------------------------------------------------------------------------------------------
 // GEMM planning / dispatch
 // ---------------------------------------------------------------------------------------------
-static GemmPlan make_plan(int n_rows, int K, int sm_count) {
+static GemmPlan make_plan(int n_rows, int K) {
   GemmPlan p;
   p.n_tiles = n_rows / 16;
   p.K = K;
   p.nsb = K / 32;
-  (void)sm_count;
   return p;
 }
 
@@ -256,7 +277,6 @@ struct GemmSched {
   bool ok = false;
 };
 static GemmSched plan_sched(int NT, int M, int pro, int epi, const GemmPlan& p, int sm_count) {
-  constexpr int fixed_ring = 0;
   GemmSched best;
   for (int want = 1; want <= 16; ++want) {
     // RMSNorm prologue: whole rows resident whenever that fits; otherwise (16-row blocks at hidden
@@ -267,9 +287,7 @@ static GemmSched plan_sched(int NT, int M, int pro, int epi, const GemmPlan& p, 
     const int n_chunks = (p.nsb + kc - 1) / kc;
     const int tpp = n_chunks > 1 ? kMaxTilesPerPass : 1;
     const GemmScratch L = gemm_scratch_layout(NT, M, kc * 32, tpp, epi);
-    const int st_hi = fixed_ring > 0 ? fixed_ring : kMaxStages;
-    const int st_lo = fixed_ring > 0 ? fixed_ring : 2;
-    for (int st = st_hi; st >= st_lo; --st) {
+    for (int st = kMaxStages; st >= 2; --st) {
       if (gemm_smem_total(st, L.total) <= (size_t)kSmemMax) {
         if (!best.ok || st > best.n_stages) {
           best.ok = true; best.tpp = tpp; best.n_chunks = n_chunks; best.kc_sbs = kc;
@@ -278,7 +296,7 @@ static GemmSched plan_sched(int NT, int M, int pro, int epi, const GemmPlan& p, 
         break;
       }
     }
-    if (best.ok && (fixed_ring > 0 || best.n_stages >= 5)) break;   // >= 80 KiB in flight per SM
+    if (best.ok && best.n_stages >= 5) break;   // >= 80 KiB in flight per SM
   }
   if (best.ok) {
     const int n_slots = (p.n_tiles + best.tpp - 1) / best.tpp;
@@ -286,9 +304,8 @@ static GemmSched plan_sched(int NT, int M, int pro, int epi, const GemmPlan& p, 
     // Tile quantisation: with g CTAs the kernel lasts ceil(n_slots / g) slot-times.  Among the
     // CTA counts that reach the minimum number of waves, take the SMALLEST one that wastes the
     // fewest slots (e.g. 768 tiles: 128 CTAs x 6 instead of 132 CTAs of which 108 run a 6th tile
-    // alone) — the TMA ring lets ~85 % of the SMs saturate HBM (LSK_GRID_EVEN=0 disables).
-    static const bool even = !(getenv("LSK_GRID_EVEN") && atoi(getenv("LSK_GRID_EVEN")) == 0);
-    if (even && fixed_ring == 0 && n_slots > sm_count) {
+    // alone) — the TMA ring lets ~85 % of the SMs saturate HBM.
+    if (n_slots > sm_count) {
       const int waves = (n_slots + sm_count - 1) / sm_count;
       int g = (n_slots + waves - 1) / waves;          // smallest CTA count with that many waves
       const int lo = sm_count * 4 / 5;
@@ -299,21 +316,7 @@ static GemmSched plan_sched(int NT, int M, int pro, int epi, const GemmPlan& p, 
   return best;
 }
 
-template <int NT, int PRO, int EPI>
-static int launch_gemm_t(lsk_engine* e, const GemmPlan& p, GemmArgs& a) {
-  // the attribute is per DEVICE: one process may drive engines on several GPUs
-  static std::atomic<uint64_t> configured{0};
-  auto kern = gemm_skinny_kernel<NT, PRO, EPI>;
-  int dev = 0;
-  CU(cudaGetDevice(&dev));
-  const uint64_t bit = 1ull << (dev & 63);
-  if (!(configured.load(std::memory_order_relaxed) & bit)) {
-    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-    configured.fetch_or(bit, std::memory_order_relaxed);
-  }
-  const GemmSched sc = plan_sched(NT, a.M, PRO, EPI, p, e->sm_count);
-  if (!sc.ok)
-    return fail(LSK_ERR_INVALID, "skinny GEMM does not fit shared memory (K=%d, NT=%d)", p.K, NT);
+static void apply_sched(GemmArgs& a, const GemmPlan& p, const GemmSched& sc) {
   a.n_tiles = p.n_tiles;
   a.nsb = p.nsb;
   a.K = p.K;
@@ -322,7 +325,16 @@ static int launch_gemm_t(lsk_engine* e, const GemmPlan& p, GemmArgs& a) {
   a.kc_sbs = sc.kc_sbs;
   a.n_stages = sc.n_stages;
   a.xs_rows = a.M;
-  CU(launch(e, kern, dim3(sc.grid), dim3(kGemmThreads), sc.smem, a));
+}
+
+template <int NT, int PRO, int EPI>
+static int launch_gemm_t(lsk_engine* e, const GemmPlan& p, GemmArgs& a) {
+  const GemmSched sc = plan_sched(NT, a.M, PRO, EPI, p, e->sm_count);
+  if (!sc.ok)
+    return fail(LSK_ERR_INVALID, "skinny GEMM does not fit shared memory (K=%d, NT=%d)", p.K, NT);
+  apply_sched(a, p, sc);
+  CU((allow_max_smem<gemm_skinny_kernel<NT, PRO, EPI>>()));
+  CU(launch(e, gemm_skinny_kernel<NT, PRO, EPI>, dim3(sc.grid), dim3(kGemmThreads), sc.smem, a));
   return LSK_OK;
 }
 
@@ -346,19 +358,9 @@ static int ll_grid(int n2, int sm_count) {
 }
 static int emit_allreduce_resid_nccl(lsk_engine* e, float* buf, float* x, int M) {
   const lsk_config& c = e->cfg;
-  e->cur_class = CLS_COMM;
-  cudaEvent_t ea = nullptr, eb = nullptr;
-  if (e->profiling) {
-    cudaEventCreate(&ea); cudaEventCreate(&eb);
-    cudaEventRecord(ea, e->stream);
-  }
-  e->launches += 1;
-  e->capture_launches += 1;
-  NC(ncclAllReduce(buf, buf, (size_t)M * c.hidden, ncclFloat, ncclSum, e->comm, e->stream));
-  if (e->profiling) {
-    cudaEventRecord(eb, e->stream);
-    e->prof_events.push_back({CLS_COMM, {ea, eb}});
-  }
+  NC(stream_op(e, CLS_COMM, [&]() {
+    return ncclAllReduce(buf, buf, (size_t)M * c.hidden, ncclFloat, ncclSum, e->comm, e->stream);
+  }));
   e->cur_class = CLS_MISC;
   CU(launch(e, residual_add_kernel, dim3(8, M), dim3(256), 0, x, c.hidden, (const float*)buf, c.hidden, c.hidden));
   return LSK_OK;
@@ -391,20 +393,14 @@ static int emit_gemm_push_resid(lsk_engine* e, const GemmPlan& p, GemmArgs a, fl
   const int NT = a.M <= 8 ? 1 : 2;
   const GemmSched sc = plan_sched(NT, a.M, PRO_BF16, EPI_PUSH, p, e->sm_count);
   if (!sc.ok) return fail(LSK_ERR_INVALID, "skinny GEMM does not fit shared memory (K=%d, NT=%d)", p.K, NT);
-  a.n_tiles = p.n_tiles; a.nsb = p.nsb; a.K = p.K;
-  a.tiles_per_pass = sc.tpp; a.n_chunks = sc.n_chunks; a.kc_sbs = sc.kc_sbs; a.n_stages = sc.n_stages;
-  a.xs_rows = a.M;
-  static std::atomic<uint64_t> configured{0};
-  int dev = 0;
-  CU(cudaGetDevice(&dev));
-  const uint64_t bit = 1ull << (dev & 63);
-  if (!(configured.load(std::memory_order_relaxed) & bit)) {
-    CU(cudaFuncSetAttribute(gemm_skinny_push_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-    CU(cudaFuncSetAttribute(gemm_skinny_push_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-    configured.fetch_or(bit, std::memory_order_relaxed);
+  apply_sched(a, p, sc);
+  if (NT == 1) {
+    CU(allow_max_smem<gemm_skinny_push_kernel<1>>());
+    CU(launch(e, gemm_skinny_push_kernel<1>, dim3(sc.grid), dim3(kGemmThreads), sc.smem, a, e->peer));
+  } else {
+    CU(allow_max_smem<gemm_skinny_push_kernel<2>>());
+    CU(launch(e, gemm_skinny_push_kernel<2>, dim3(sc.grid), dim3(kGemmThreads), sc.smem, a, e->peer));
   }
-  if (NT == 1) CU(launch(e, gemm_skinny_push_kernel<1>, dim3(sc.grid), dim3(kGemmThreads), sc.smem, a, e->peer));
-  else CU(launch(e, gemm_skinny_push_kernel<2>, dim3(sc.grid), dim3(kGemmThreads), sc.smem, a, e->peer));
   e->cur_class = CLS_COMM;
   const int n2 = a.M * c.hidden / 2;
   CU(launch(e, tp_finish_ll_kernel, dim3(ll_grid(n2, e->sm_count)), dim3(kArThreads), 0, e->peer, x, n2));
@@ -441,17 +437,8 @@ static AttnLaunchPlan plan_attention_launch(int head_dim, int group, int M, int 
 // pz: the piece grid (kv heads, splits, pieces) of attn_piece_kernel, with a.M the largest piece's rows.
 template <int HD>
 static int launch_attention_t(lsk_engine* e, AttnArgs& a, const AttnPieces* pz, int n_pieces) {
-  static std::atomic<uint64_t> configured{0};
-  int dev = 0;
-  CU(cudaGetDevice(&dev));
-  const uint64_t bit = 1ull << (dev & 63);
-  if (!(configured.load(std::memory_order_relaxed) & bit)) {
-    CU(cudaFuncSetAttribute(attn_split_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-    CU(cudaFuncSetAttribute(attn_piece_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
-    configured.fetch_or(bit, std::memory_order_relaxed);
-  }
   const int grid_z = pz ? n_pieces : 1;
-  const AttnLaunchPlan lp = plan_attention_launch(HD, a.group, a.M, a.n_kv_heads * grid_z, a.n_splits, e->attn_stages,
+  const AttnLaunchPlan lp = plan_attention_launch(HD, a.group, a.M, a.n_kv_heads * grid_z, a.n_splits, kAttnMaxStages,
                                                   e->sm_count);
   const AttnSmemPlan& sp = lp.sp;
   a.n_stages = lp.stages;
@@ -462,33 +449,15 @@ static int launch_attention_t(lsk_engine* e, AttnArgs& a, const AttnPieces* pz, 
   if (attn_part_floats(a.n_kv_heads, a.n_splits, pz ? pz->part_rows : a.rows_pad, HD) > e->attn_part_cap)
     return fail(LSK_ERR_INVALID, "attention: %d query rows per kv head exceed the partials buffer", a.group * a.M);
   a.part = e->attn_part; a.arrive = pz ? e->piece_arrive : e->attn_arrive;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(a.n_kv_heads, a.n_splits, grid_z);
-  cfg.blockDim = dim3(kAttnThreads);
-  // a grid that fits one wave gets a whole SM per CTA (> half of the SM's shared memory): the
-  // CTAs then spread over the SMs instead of sharing a few SMs' load bandwidth
-  cfg.dynamicSmemBytes = lp.smem;
-  cfg.stream = e->stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = e->use_pdl ? 1 : 0;
-  e->launches += 1;
-  e->capture_launches += 1;
-  auto go = [&]() {
-    return pz ? cudaLaunchKernelEx(&cfg, attn_piece_kernel<HD>, a, *pz) : cudaLaunchKernelEx(&cfg, attn_split_kernel<HD>, a);
-  };
-  if (!e->profiling) {
-    CU(go());
+  // lp.smem: a grid that fits one wave gets a whole SM per CTA (> half of the SM's shared memory):
+  // the CTAs then spread over the SMs instead of sharing a few SMs' load bandwidth
+  const dim3 grid(a.n_kv_heads, a.n_splits, grid_z);
+  if (pz) {
+    CU(allow_max_smem<attn_piece_kernel<HD>>());
+    CU(launch(e, attn_piece_kernel<HD>, grid, dim3(kAttnThreads), lp.smem, a, *pz));
   } else {
-    cudaEvent_t ea, eb;
-    cudaEventCreate(&ea); cudaEventCreate(&eb);
-    cudaEventRecord(ea, e->stream);
-    cudaError_t err = go();
-    cudaEventRecord(eb, e->stream);
-    e->prof_events.push_back({e->cur_class, {ea, eb}});
-    CU(err);
+    CU(allow_max_smem<attn_split_kernel<HD>>());
+    CU(launch(e, attn_split_kernel<HD>, grid, dim3(kAttnThreads), lp.smem, a));
   }
   return LSK_OK;
 }
@@ -515,16 +484,13 @@ static int alloc_attn_partials(lsk_engine* e, int kv_heads, int group, int head_
 // one decoder layer on hidden rows [row0, row0 + M) at positions *base_len + pos_off + i
 //   (HF LlamaDecoderLayer as called at llama_model_utils.py:193-201,253-261,354-362,375-383)
 // ---------------------------------------------------------------------------------------------
-static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base_len, int pos_off,
-                         const void* after_W = nullptr, size_t after_bytes = 0) {
+static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base_len, int pos_off) {
   const lsk_config& c = e->cfg;
   LayerWeights& L = e->layers[li];
   float* x = e->hidden + (size_t)row0 * c.hidden;
   __nv_bfloat16* kp = e->kpool + (size_t)li * e->pool_layer_elems;
   __nv_bfloat16* vp = e->vpool + (size_t)li * e->pool_layer_elems;
   const bool tp = c.tp_size > 1;
-  const size_t h2 = (size_t)c.hidden * 2;
-  auto cap = [&](size_t bytes) { return bytes < e->l2_prefetch_bytes ? bytes : e->l2_prefetch_bytes; };
 
   if (!(e->ablate & (1u << CLS_QKV))) {  // RMSNorm -> QKV -> RoPE -> KV append
     e->cur_class = CLS_QKV;
@@ -536,7 +502,6 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
     a.kpool = kp; a.vpool = vp; a.page_table = e->page_table;
     a.base_len = base_len; a.pos_off = pos_off; a.rope = e->rope; a.head_dim = c.head_dim;
     a.q_rows = e->q_rows; a.kv_rows = e->kv_rows; a.n_kv_heads = e->kv_heads_l;
-    a.next_W = L.wo; a.next_bytes = e->l2_prefetch_bytes ? (size_t)e->q_rows * h2 : 0;
     TRY((launch_gemm<PRO_RMS, EPI_QKV>(e, e->p_qkv, a)));
   }
   if (!(e->ablate & (1u << CLS_ATTN))) {  // attention over the paged cache
@@ -555,7 +520,6 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
     a.W = reinterpret_cast<const uint4*>(L.wo);
     a.M = M;
     a.x_bf16 = e->attn_out; a.xb_ld = e->q_rows;
-    a.next_W = L.wgu; a.next_bytes = cap((size_t)2 * e->inter_l * h2);
     if (!tp) {
       a.out_f32 = x; a.out_ld = c.hidden;
       TRY((launch_gemm<PRO_BF16, EPI_RESID>(e, e->p_o, a)));
@@ -574,7 +538,6 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
     a.M = M;
     a.x_f32 = x; a.x_ld = c.hidden; a.norm_w = L.ln2; a.eps = c.rms_eps;
     a.act = e->act; a.act_ld = e->inter_l_pad;
-    a.next_W = L.wd; a.next_bytes = cap((size_t)e->inter_l * h2);
     TRY((launch_gemm<PRO_RMS, EPI_SILU>(e, e->p_gu, a)));
   }
   if (!(e->ablate & (1u << CLS_DOWN))) {  // down projection (+ residual)
@@ -583,7 +546,6 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
     a.W = reinterpret_cast<const uint4*>(L.wd);
     a.M = M;
     a.x_bf16 = e->act; a.xb_ld = e->inter_l_pad;
-    a.next_W = after_W; a.next_bytes = after_W ? cap(after_bytes) : 0;
     if (!tp) {
       a.out_f32 = x; a.out_ld = c.hidden;
       TRY((launch_gemm<PRO_BF16, EPI_RESID>(e, e->p_d, a)));
@@ -684,9 +646,9 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool c
     e->cur_class = CLS_COMM;
     CU(launch(e, reduce_partials_kernel, dim3(m), dim3(256), 0, (const float*)e->part_p, n_splits, part_stride,
               c.hidden, c.hidden, e->tp_buf_p));
-    e->launches += 1;
-    e->capture_launches += 1;
-    NC(ncclAllReduce(e->tp_buf_p, e->tp_buf_p, (size_t)m * c.hidden, ncclFloat, ncclSum, e->comm, e->stream));
+    NC(stream_op(e, CLS_COMM, [&]() {
+      return ncclAllReduce(e->tp_buf_p, e->tp_buf_p, (size_t)m * c.hidden, ncclFloat, ncclSum, e->comm, e->stream);
+    }));
     pend = e->tp_buf_p; n_pend = 1;
     return LSK_OK;
   };
@@ -788,23 +750,22 @@ static int emit_finalize(lsk_engine* e, int slot, float* dst_row) {
 }
 // token history (prompt ids + emitted tokens) is kept on the device only when the n-gram ban needs it
 static int* hist_ptr(lsk_engine* e) { return e->gen.no_repeat_ngram_size > 0 ? e->d_prompt : nullptr; }
-static int emit_accept(lsk_engine* e, int d_spec, int seq) {
+static int emit_accept(lsk_engine* e, int d_spec) {
   e->cur_class = CLS_MISC;
   CU(launch(e, accept_greedy_kernel, dim3(1), dim3(256), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e), d_spec,
-            e->state, (const GenParams*)e->gen_dev, e->res_dev, seq, hist_ptr(e)));
+            e->state, (const GenParams*)e->gen_dev, e->res_dev, 0, hist_ptr(e)));
   return LSK_OK;
 }
-static int emit_ar_commit(lsk_engine* e, int seq) {
+static int emit_ar_commit(lsk_engine* e) {
   e->cur_class = CLS_MISC;
   CU(launch(e, ar_commit_kernel, dim3(1), dim3(32), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e), e->state,
-            e->res_dev, seq, hist_ptr(e)));
+            e->res_dev, 0, hist_ptr(e)));
   return LSK_OK;
 }
 
 // Final RMSNorm + the mma.sync LM head on M fp32 residual rows at x (row stride hidden): arg-max
 // candidates into cand_*, and the logits rows when `logits` is set.
-static int launch_lm_head_gemm(lsk_engine* e, const float* x, int M, float* logits, const void* after_W = nullptr,
-                               size_t after_bytes = 0) {
+static int launch_lm_head_gemm(lsk_engine* e, const float* x, int M, float* logits) {
   const lsk_config& c = e->cfg;
   GemmArgs a{};
   a.W = reinterpret_cast<const uint4*>(e->lm_head);
@@ -814,8 +775,6 @@ static int launch_lm_head_gemm(lsk_engine* e, const float* x, int M, float* logi
   a.logits = logits; a.logits_ld = e->vocab_l_pad;
   a.n_valid_rows = e->vocab_l; a.vocab_off = e->vocab_off;
   a.part_val = e->cand_val; a.part_idx = e->cand_idx;
-  a.next_W = after_W;
-  a.next_bytes = after_W ? (after_bytes < e->l2_prefetch_bytes ? after_bytes : e->l2_prefetch_bytes) : 0;
   return launch_gemm<PRO_RMS, EPI_LMHEAD>(e, e->p_lm, a);
 }
 
@@ -826,7 +785,7 @@ static int launch_lm_head_gemm(lsk_engine* e, const float* x, int M, float* logi
 // are materialised, the tokens that would repeat an n-gram of the sequence so far are set to -inf
 // (row r continues prompt ++ output ++ draft[0 .. j0 + r)), and the arg-max is taken from the
 // banned rows instead of the LM-head epilogue.
-static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0, const void* after_W = nullptr, size_t after_bytes = 0) {
+static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0) {
   const lsk_config& c = e->cfg;
   const bool ban = e->gen.no_repeat_ngram_size > 0;
   e->cur_class = CLS_LMHEAD;
@@ -842,7 +801,7 @@ static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0, const void* a
       CU(launch(e, lmhead_tc_kernel, dim3(e->lm_tc_grid), dim3(kTcThreads),
                 lmhead_tc_smem_bytes(c.hidden, e->lm_tc_stages), t));
     }
-  } else if (!(e->ablate & (1u << CLS_LMHEAD))) TRY(launch_lm_head_gemm(e, x, M, logits, after_W, after_bytes));
+  } else if (!(e->ablate & (1u << CLS_LMHEAD))) TRY(launch_lm_head_gemm(e, x, M, logits));
   e->cur_class = CLS_MISC;
   const float* cv = e->cand_val;
   const int* ci = e->cand_idx;
@@ -862,7 +821,8 @@ static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0, const void* a
   e->cur_cand_val = cv; e->cur_cand_idx = ci; e->cur_n_cand = ncand;
   if (c.tp_size > 1 && e->gen.sample) {
     // every rank needs the whole distribution: all-gather the vocab shards of the M rows, lay them
-    // out as [M][vocab]; all ranks then run the same warp / Philox draw and stay in lockstep
+    // out as [M][vocab]; all ranks then run the same warp / Philox draw and stay in lockstep.
+    // (The all-gathers of this function are not counted as launches, unlike the all-reduces.)
     e->cur_class = CLS_COMM;
     NC(ncclAllGather(e->logits, e->logits_gath, (size_t)M * e->vocab_l_pad, ncclFloat, e->comm, e->stream));
     CU(launch(e, tp_logits_rows_kernel, dim3(32, M), dim3(256), 0, (const float*)e->logits_gath, c.tp_size, M,
@@ -886,24 +846,16 @@ static int n_cand(lsk_engine* e) { return e->cfg.tp_size > 1 ? e->cfg.tp_size : 
 // ---------------------------------------------------------------------------------------------
 // round / AR-step command streams
 // ---------------------------------------------------------------------------------------------
-static int enqueue_round(lsk_engine* e, int E, int d, int seq) {
+static int enqueue_round(lsk_engine* e, int E, int d) {
   const lsk_config& c = e->cfg;
   const int* len = &e->state->len;
   // row 0 <- embedding of the pending token (self_speculation_generator.py:122, input_ids)
   TRY(emit_embed(e, &e->state->tok[0], e->hidden, 1));
   // draft loop (:127-148): step i runs layers [0,E) on row i at position len+i, then the shared
   // head; its arg-max becomes tok[i+1] and is embedded into row i+1.
-  const size_t qkv_bytes = (size_t)(e->q_rows + 2 * e->kv_rows) * c.hidden * 2;
-  const size_t lm_bytes = (size_t)e->vocab_l_pad * c.hidden * 2;
-  auto layer_then = [&](int l, int row0, int M, int pos_off, int stop) -> int {
-    // what streams after layer l: the next layer's QKV, or the LM head at the end of a pass
-    const void* nw = (l + 1 < stop) ? (const void*)e->layers[l + 1].wqkv : (const void*)e->lm_head;
-    const size_t nb = (l + 1 < stop) ? qkv_bytes : lm_bytes;
-    return enqueue_layer(e, l, row0, M, len, pos_off, nw, nb);
-  };
   for (int i = 0; i < d; ++i) {
-    for (int l = 0; l < E; ++l) TRY(layer_then(l, i, 1, i, E));
-    TRY(enqueue_lm_head(e, i, 1, i, e->layers[0].wqkv, qkv_bytes));
+    for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, i, 1, len, i));
+    TRY(enqueue_lm_head(e, i, 1, i));
     e->cur_class = CLS_MISC;
     if (!e->gen.sample) {
       TRY(emit_finalize(e, 1 + i, e->hidden + (size_t)(i + 1) * c.hidden));
@@ -919,52 +871,44 @@ static int enqueue_round(lsk_engine* e, int E, int d, int seq) {
   }
   // verify (:164-174 -> llama_model_utils.py:280-391): the last drafted token has not been
   // through layers < E yet (:350-362) ...
-  for (int l = 0; l < E; ++l) {
-    if (l + 1 < E || E < c.n_layers) TRY(enqueue_layer(e, l, d, 1, len, d, e->layers[l + 1].wqkv, qkv_bytes));
-    else TRY(enqueue_layer(e, l, d, 1, len, d, e->lm_head, lm_bytes));
-  }
+  for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, d, 1, len, d));
   // ... then layers >= E see [exit rows of the draft steps ; that row] = rows 0..d (:363-383)
-  for (int l = E; l < c.n_layers; ++l) TRY(layer_then(l, 0, d + 1, 0, c.n_layers));
-  TRY(enqueue_lm_head(e, 0, d + 1, 0, e->layers[0].wqkv, qkv_bytes));
+  for (int l = E; l < c.n_layers; ++l) TRY(enqueue_layer(e, l, 0, d + 1, len, 0));
+  TRY(enqueue_lm_head(e, 0, d + 1, 0));
   e->cur_class = CLS_MISC;
   if (!e->gen.sample) {
-    TRY(emit_accept(e, d, seq));
+    TRY(emit_accept(e, d));
   } else {
     CU(launch(e, warp_and_sample_kernel, dim3(d + 1), dim3(kSampleThreads), 0, samp_logits(e),
               samp_ld(e), c.vocab, (const GenParams*)e->gen_dev, (const DevState*)e->state,
               e->probs_v, &e->state->verified[0], (int)RNG_VERIFY, 0));
     CU(launch(e, accept_sample_kernel, dim3(1), dim3(kSampleThreads), 0, (const float*)e->probs_d,
               (const float*)e->probs_v, c.vocab, d, e->state, (const GenParams*)e->gen_dev, e->res_dev,
-              e->samp_scratch, seq, hist_ptr(e)));
+              e->samp_scratch, 0, hist_ptr(e)));
   }
   return LSK_OK;
 }
 
-static int enqueue_ar(lsk_engine* e, int n_layers_run, int seq) {
+static int enqueue_ar(lsk_engine* e, int n_layers_run) {
   const lsk_config& c = e->cfg;
   const int* len = &e->state->len;
   TRY(emit_embed(e, &e->state->tok[0], e->hidden, 1));
-  const size_t qkv_bytes = (size_t)(e->q_rows + 2 * e->kv_rows) * c.hidden * 2;
-  const size_t lm_bytes = (size_t)e->vocab_l_pad * c.hidden * 2;
-  for (int l = 0; l < n_layers_run; ++l) {
-    if (l + 1 < n_layers_run) TRY(enqueue_layer(e, l, 0, 1, len, 0, e->layers[l + 1].wqkv, qkv_bytes));
-    else TRY(enqueue_layer(e, l, 0, 1, len, 0, e->lm_head, lm_bytes));
-  }
-  TRY(enqueue_lm_head(e, 0, 1, 0, e->layers[0].wqkv, qkv_bytes));
+  for (int l = 0; l < n_layers_run; ++l) TRY(enqueue_layer(e, l, 0, 1, len, 0));
+  TRY(enqueue_lm_head(e, 0, 1, 0));
   e->cur_class = CLS_MISC;
   if (!e->gen.sample) {
-    TRY(emit_ar_commit(e, seq));
+    TRY(emit_ar_commit(e));
   } else {
     CU(launch(e, warp_and_sample_kernel, dim3(1), dim3(kSampleThreads), 0, samp_logits(e),
               samp_ld(e), c.vocab, (const GenParams*)e->gen_dev, (const DevState*)e->state,
               e->probs_v, &e->state->verified[0], (int)RNG_VERIFY, 0));
-    CU(launch(e, ar_commit_sampled_kernel, dim3(1), dim3(32), 0, e->state, e->res_dev, seq, hist_ptr(e)));
+    CU(launch(e, ar_commit_sampled_kernel, dim3(1), dim3(32), 0, e->state, e->res_dev, 0, hist_ptr(e)));
   }
   return LSK_OK;
 }
 
-// Run `enqueue` either eagerly or as a cached CUDA graph keyed by `key`.  The completion stamp
-// (`seq`) is baked into eager launches; graph replays use stamp 0 + an event instead.
+// Run `enqueue` either eagerly or as a cached CUDA graph keyed by `key`.  Completion is
+// the ev1 event in both modes; the commit kernels' stamp (RoundResult::seq) is always 0.
 template <typename F>
 static int run_cached(lsk_engine* e, long long key, F enqueue) {
   CU(cudaEventRecord(e->ev0, e->stream));
@@ -1089,19 +1033,14 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
   // ONE CTA per SM on as many SMs as possible — splits = floor(SMs / kv heads), at most 4 (7B: 32
   // heads x 4 splits; an 8-way split's merge costs more than extra SMs bring).
   e->n_splits = c.attn_splits > 0 ? c.attn_splits : attn_default_splits(e->sm_count, e->kv_heads_l);
-  if (const char* env = getenv("LSK_ATTN_SPLITS")) e->n_splits = atoi(env);   // clamped to [1, 8] below
-  if (const char* env = getenv("LSK_ATTN_STAGES")) e->attn_stages = atoi(env);
-  if (e->attn_stages < 2) e->attn_stages = 2;
-  if (e->attn_stages > kAttnMaxStages) e->attn_stages = kAttnMaxStages;
   if (e->n_splits > 8) e->n_splits = 8;
   if (e->n_splits < 1) e->n_splits = 1;
 
-  e->p_qkv = make_plan(e->q_rows + 2 * e->kv_rows, c.hidden, e->sm_count);
-  e->p_o = make_plan(c.hidden, e->q_rows, e->sm_count);
-  e->p_gu = make_plan(2 * e->inter_l, c.hidden, e->sm_count);
-  e->p_d = make_plan(c.hidden, e->inter_l_pad, e->sm_count);
-  e->p_lm = make_plan(e->vocab_l_pad, c.hidden, e->sm_count);
-  if (const char* env = getenv("LSK_L2_PREFETCH_MB")) e->l2_prefetch_bytes = (size_t)atoi(env) << 20;
+  e->p_qkv = make_plan(e->q_rows + 2 * e->kv_rows, c.hidden);
+  e->p_o = make_plan(c.hidden, e->q_rows);
+  e->p_gu = make_plan(2 * e->inter_l, c.hidden);
+  e->p_d = make_plan(c.hidden, e->inter_l_pad);
+  e->p_lm = make_plan(e->vocab_l_pad, c.hidden);
   if (getenv("LSK_LMHEAD_TC") && atoi(getenv("LSK_LMHEAD_TC")) != 0) {
     // wgmma LM head: needs hidden % 64 == 0 and the 16-token B operand + a >= 3-stage ring in
     // shared memory (hidden <= 5120); otherwise stay on the mma.sync kernel, loudly
@@ -1551,9 +1490,7 @@ int lsk_prefill(lsk_engine* e, const int32_t* ids, int32_t n) {
       const int m = (n - 1 - c0) < e->max_rows ? (n - 1 - c0) : e->max_rows;
       CU(launch(e, embed_tokens_kernel, dim3(m), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
                 (const int*)(e->d_prompt + c0), e->hidden, c.hidden));
-      for (int l = 0; l < c.n_layers; ++l)
-        TRY(enqueue_layer(e, l, 0, m, e->d_zero, c0, e->layers[(l + 1) % c.n_layers].wqkv,
-                          (size_t)(e->q_rows + 2 * e->kv_rows) * c.hidden * 2));
+      for (int l = 0; l < c.n_layers; ++l) TRY(enqueue_layer(e, l, 0, m, e->d_zero, c0));
     }
   }
   set_state_kernel<<<1, 1, 0, e->stream>>>(e->state, n - 1, ids[n - 1], 0, n);
@@ -1587,11 +1524,9 @@ int lsk_round(lsk_engine* e, int32_t d_req, lsk_round_out* out) {
   const int E = e->gen.exit_layer;
   if (E < 1 || E > e->cfg.n_layers) return fail(LSK_ERR_INVALID, "self-speculation needs 1 <= exit_layer <= n_layers (got %d)", E);
   if (e->host_len + d_req + 2 > e->max_pos) return fail(LSK_ERR_CTX, "context %d + %d exceeds max_ctx", e->host_len, d_req + 1);
-  const int seq = ++e->seq;
   const long long key = ((long long)E << 20) | ((long long)d_req << 8) | (e->gen.sample ? 4 : 0) | 1 |
                         ((long long)e->gen.no_repeat_ngram_size << 32);
-  TRY(run_cached(e, key, [&]() { return enqueue_round(e, E, d_req, 0); }));
-  (void)seq;
+  TRY(run_cached(e, key, [&]() { return enqueue_round(e, E, d_req); }));
   TRY(peer_check(e));
   copy_result(e, out);
   e->host_len = out->kv_len;
@@ -1604,7 +1539,7 @@ int lsk_ar_step(lsk_engine* e, int32_t* token_out) {
   if (e->host_len + 2 > e->max_pos) return fail(LSK_ERR_CTX, "context exceeds max_ctx");
   const int nl = (e->gen.exit_layer > 0 && e->gen.exit_layer <= e->cfg.n_layers) ? e->gen.exit_layer : e->cfg.n_layers;
   const long long key = ((long long)nl << 20) | (e->gen.sample ? 4 : 0) | 2 | ((long long)e->gen.no_repeat_ngram_size << 32);
-  TRY(run_cached(e, key, [&]() { return enqueue_ar(e, nl, 0); }));
+  TRY(run_cached(e, key, [&]() { return enqueue_ar(e, nl); }));
   TRY(peer_check(e));
   *token_out = e->res_host->emitted_ids[0];
   e->host_len = e->res_host->kv_len;
@@ -1622,7 +1557,7 @@ int lsk_profile_round(lsk_engine* e, int32_t d_req, lsk_round_out* out, float* c
   e->profiling = true;
   e->prof_events.clear();
   CU(cudaEventRecord(e->ev0, e->stream));
-  int st = enqueue_round(e, E, d_req, 0);
+  int st = enqueue_round(e, E, d_req);
   e->profiling = false;
   if (st != LSK_OK) return st;
   CU(cudaEventRecord(e->ev1, e->stream));
@@ -2117,7 +2052,7 @@ int lsk_plan_gemm(int64_t n_rows, int64_t K, int32_t m, int32_t pro, int32_t epi
                   lsk_gemm_plan* out) {
   if (!out || n_rows % 16 || K % 32 || m < 1 || m > kMaxRows || sm_count < 1)
     return fail(LSK_ERR_INVALID, "bad plan query");
-  const GemmPlan p = make_plan((int)n_rows, (int)K, sm_count);
+  const GemmPlan p = make_plan((int)n_rows, (int)K);
   const int NT = m <= 8 ? 1 : 2;
   const GemmSched sc = plan_sched(NT, m, pro, epi, p, sm_count);
   out->ok = sc.ok ? 1 : 0;
@@ -2177,7 +2112,7 @@ int lsk_test_gemm(const void* packed, int64_t n, int64_t k, const void* x, int32
   CU(cudaDeviceGetAttribute(&tmp.sm_count, cudaDevAttrMultiProcessorCount, dev));
   CU(cudaStreamCreateWithFlags(&tmp.stream, cudaStreamNonBlocking));
   tmp.use_pdl = true;
-  GemmPlan p = make_plan((int)n, (int)k, tmp.sm_count);
+  GemmPlan p = make_plan((int)n, (int)k);
   GemmArgs a{};
   a.W = (const uint4*)packed;
   a.M = m;

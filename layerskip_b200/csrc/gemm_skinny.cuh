@@ -54,10 +54,6 @@ __device__ __forceinline__ void bar_sync(int id, int n) {
 __device__ __forceinline__ void bar_arrive(int id, int n) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory");
 }
-// fire-and-forget: pull [p, p+bytes) into L2 (bytes % 16 == 0)
-__device__ __forceinline__ void l2_prefetch_bulk(const void* p, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
 struct GemmArgs {
   const uint4* W;       // packed weights
   int n_tiles;          // N / 16
@@ -70,9 +66,6 @@ struct GemmArgs {
   int kc_sbs;           // super-blocks per chunk (multiple of kStageSbs unless n_chunks == 1)
   int n_stages;         // ring depth
   int xs_rows;          // activation rows resident in shared memory (= M; absent rows read as 0)
-  // ---- next kernel's weights: its head is pulled into L2 while this kernel drains
-  const void* next_W;
-  unsigned long long next_bytes;   // bytes worth prefetching (0 = none)
   // ---- prologue
   const float* x_f32;   // PRO_RMS: residual-stream rows [M][x_ld] fp32
   int x_ld;
@@ -490,22 +483,6 @@ __device__ __forceinline__ void gemm_epilogue_role(const GemmArgs& a, const Gemm
   int it = 0;
   for (int slot = blockIdx.x; slot < n_slots; slot += gridDim.x, ++it) {
     const int buf = it & 1;
-    const bool last = slot + gridDim.x >= n_slots;
-    if (last && a.next_bytes != 0) {
-      // HBM keeps streaming while this kernel drains and the next one ramps up
-      const unsigned long long share = ((a.next_bytes / gridDim.x) + 15) & ~15ull;
-      const unsigned long long lo = (unsigned long long)blockIdx.x * share;
-      if (lo < a.next_bytes) {
-        unsigned long long len = a.next_bytes - lo < share ? a.next_bytes - lo : share;
-        len &= ~15ull;
-        const unsigned long long per = ((len / kEpiThreads) + 15) & ~15ull;
-        const unsigned long long mylo = (unsigned long long)etid * per;
-        if (mylo < len && per > 0) {
-          const unsigned long long mylen = len - mylo < per ? len - mylo : per;
-          l2_prefetch_bulk(static_cast<const unsigned char*>(a.next_W) + lo + mylo, (uint32_t)mylen);
-        }
-      }
-    }
     // EPI_RESID: fetch the old residual values of this slot BEFORE waiting for the tile, so the
     // tail of the kernel has no dependent global round trip (each element has one owner thread)
     constexpr int kMaxItems = (kMaxTilesPerPass * NT * 128 + kEpiThreads - 1) / kEpiThreads;
@@ -683,7 +660,6 @@ __device__ __forceinline__ void gemm_epilogue_role(const GemmArgs& a, const Gemm
 template <int NT, int PRO, int EPI>
 __device__ __forceinline__ void gemm_work(const GemmArgs& a, const GemmCtx& c, uint32_t& q,
                                           int tid, int warp, int lane,
-                                          unsigned long long* phase_clk = nullptr,
                                           const uint2* pre_wreg = nullptr,
                                           const PeerComm* pc = nullptr) {
   const int wtid = (warp < kGemmWarps) ? tid : tid - 32;   // 0..607 over consumers + epilogue
@@ -698,16 +674,14 @@ __device__ __forceinline__ void gemm_work(const GemmArgs& a, const GemmCtx& c, u
     }
   }
   gemm_prologue<NT, PRO>(a, c, EPI, wtid, swarp, lane, wreg);
-  if (phase_clk != nullptr && wtid == 0) phase_clk[1] = clock64();      // debug: prologue done
   if (warp < kGemmWarps) gemm_consume<NT>(a, c, EPI, q, tid, warp, lane);
   else gemm_epilogue_role<NT, EPI>(a, c, tid - kConsumerThreads - 32, warp - kGemmWarps - 1, lane, pc);
-  if (phase_clk != nullptr && wtid == 0) phase_clk[2] = clock64();      // debug: my tiles consumed
 }
 
 // Stand-alone kernel (one CTA per SM, persistent over tiles; 20 warps):
 //   warp 16      : PRODUCER (starts before the previous kernel has finished: PDL)
 //   warps 0..15  : CONSUMERS
-//   warps 17..19 : EPILOGUE (+ L2 prefetch of the NEXT kernel's first weights at the end)
+//   warps 17..19 : EPILOGUE
 template <int NT, int PRO, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_skinny_kernel(const GemmArgs a) {
@@ -727,7 +701,7 @@ gemm_skinny_kernel(const GemmArgs a) {
   uint2 wreg[4];
   if (PRO == PRO_RMS) gemm_preload_norm(a, (warp < kGemmWarps) ? tid : tid - 32, wreg);
   pdl_wait();
-  gemm_work<NT, PRO, EPI>(a, c, q, tid, warp, lane, nullptr, PRO == PRO_RMS ? wreg : nullptr);
+  gemm_work<NT, PRO, EPI>(a, c, q, tid, warp, lane, PRO == PRO_RMS ? wreg : nullptr);
 }
 
 // Tensor-parallel row-parallel GEMM whose epilogue pushes its tiles to every rank (EPI_PUSH).
@@ -748,7 +722,7 @@ gemm_skinny_push_kernel(const GemmArgs a, const __grid_constant__ PeerComm pc) {
   }
   pdl_launch_dependents();
   pdl_wait();
-  gemm_work<NT, PRO_BF16, EPI_PUSH>(a, c, q, tid, warp, lane, nullptr, nullptr, &pc);
+  gemm_work<NT, PRO_BF16, EPI_PUSH>(a, c, q, tid, warp, lane, nullptr, &pc);
 }
 
 }  // namespace lsk
