@@ -177,6 +177,21 @@ int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer,
 int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
                     int32_t exit_layer, float* logprob_out, int32_t* greedy_out);
 
+/* Teacher-forced scoring of continuations that share contexts, single GPU, wgmma prompt pass
+ * required.  Prefix p is prefix_ids[prefix_offsets[p] .. prefix_offsets[p+1]-1] and branch b is
+ * branch_ids[branch_offsets[b] .. branch_offsets[b+1]-1], each at least 1 id (both offset arrays
+ * start at 0 and increase); branch b continues prefix branch_prefix[b] and scores P + B, with
+ * len(P) + len(B) <= max_ctx.  Every prefix has at least one branch; branches come in any order.
+ * Outputs have one entry per branch id, concatenated in input order (branch b owns
+ * [branch_offsets[b], branch_offsets[b+1])): entry i of branch b is the log-probability of B[i]
+ * after P + B[:i], and greedy_out (may be NULL) the arg-max token there.  These are bit-identical
+ * to entries len(P)-1 .. len(P)+len(B)-2 of lsk_score_batch of P + B.  A prefix's rows run once
+ * per group, writing K/V only; its own ids are not scored.  Same state rules as lsk_score. */
+int lsk_score_prefixed(lsk_engine* e, const int32_t* prefix_ids, const int32_t* prefix_offsets,
+                       int32_t n_prefixes, const int32_t* branch_ids, const int32_t* branch_offsets,
+                       const int32_t* branch_prefix, int32_t n_branches, int32_t exit_layer,
+                       float* logprob_out, int32_t* greedy_out);
+
 /* Teacher-forced scoring of ids[0..n-1] at n_exits exit layers in ONE pass, single GPU.  exits is
  * strictly increasing, each in [1, n_layers], 1 <= n_exits <= LSK_MAX_EXITS.  Layers below each
  * exit run once: the heads of the earlier exits run inside the pass of the deepest one.

@@ -99,6 +99,9 @@ SIGNATURES = {
                             C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
     "lsk_score_batch": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
                                   C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
+    "lsk_score_prefixed": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                     C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                     C.c_int32, C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
     "lsk_score_exits": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32), C.c_int32,
                                   C.POINTER(lsk_generation), C.POINTER(C.c_float), C.POINTER(C.c_int32),
                                   C.POINTER(C.c_float)]),

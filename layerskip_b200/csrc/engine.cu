@@ -125,6 +125,7 @@ struct lsk_engine {
   __nv_bfloat16* vpool = nullptr;
   size_t pool_layer_elems = 0;
   int* page_table = nullptr;
+  std::vector<int> page_table_host;    // host copy of page_table (prefix-shared scoring builds its views from it)
   float2* rope = nullptr;
 
   float* hidden = nullptr;             // [16][hidden] fp32 residual-stream rows
@@ -155,6 +156,7 @@ struct lsk_engine {
   int* score_greedy = nullptr;         // lsk_score: [max_pos] arg-max ids
   int* batch_buf = nullptr;            // lsk_score_batch: [8][max_pos] row ids, targets, row map, pieces of a group
   unsigned int* piece_arrive = nullptr;  // lsk_score_batch: [128 pieces][kv heads] attention arrival counters
+  int* view_table = nullptr;           // lsk_score_prefixed: [max_pos] physical pages of a group's page-table views
   // lsk_score_exits (allocated on first use, grown with the number of exits)
   int exits_cap = 0;                   // exits the result arrays hold
   float* exits_lp = nullptr;           // [exits_cap][max_pos] log-probabilities
@@ -604,11 +606,14 @@ static int launch_prompt_attention(lsk_engine* e, const __nv_bfloat16* q, int q_
 
 // A chunk of rows from several sequences (lsk_score_batch), device pointers at the chunk's first row:
 // ids, per-row (position, first logical page), and the chunk's attention pieces (AttnPieces::pieces).
+// The first pages index page_table (nullptr: the engine's page table; lsk_score_prefixed passes
+// its table of page-table views).
 struct PackedChunk {
   const int* ids;
   const int2* row_map;
   const int4* pieces;
   int n_pieces, max_piece_rows;
+  const int* page_table = nullptr;
 };
 
 // Scoring at several exits in one pass (lsk_score_exits): at the top of layer layers[t] the first
@@ -630,6 +635,7 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool c
                                  const PackedChunk* pk = nullptr, const ChunkTaps* taps = nullptr) {
   const lsk_config& c = e->cfg;
   const bool tp = c.tp_size > 1;
+  const int* pk_pages = pk && pk->page_table ? pk->page_table : e->page_table;
   e->cur_class = CLS_MISC;
   CU(launch(e, embed_tokens_kernel, dim3(m), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
             pk ? pk->ids : (const int*)(e->d_prompt + c0), e->hidden_p, c.hidden));
@@ -669,6 +675,7 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool c
       a.q_rows = e->q_rows; a.kv_rows = e->kv_rows; a.n_kv_heads = e->kv_heads_l;
       if (pk) {
         a.row_map = pk->row_map;
+        a.page_table = pk_pages;
         TRY(launch_prefill_gemm<PF_EPI_QKV_MAP>(e, a));
       } else {
         TRY(launch_prefill_gemm<PF_EPI_QKV>(e, a));
@@ -682,7 +689,7 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool c
       AttnArgs a{};
       a.q = e->q_p; a.q_ld = e->q_rows;
       a.out = reinterpret_cast<__nv_bfloat16*>(e->attn_c); a.out_canon = 1;
-      a.kpool = kp; a.vpool = vp; a.page_table = e->page_table; a.base_len = e->d_zero;
+      a.kpool = kp; a.vpool = vp; a.page_table = pk_pages; a.base_len = e->d_zero;
       a.M = pk->max_piece_rows; a.group = e->group; a.n_kv_heads = e->kv_heads_l; a.n_splits = e->n_splits;
       a.scale = 1.0f / sqrtf((float)c.head_dim);
       const AttnPieces pz{pk->pieces, (e->group * kPfTokens + 15) / 16 * 16};
@@ -1148,6 +1155,7 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
     std::vector<int> pt(e->n_pages);
     for (int i = 0; i < e->n_pages; ++i) pt[i] = i;
     CU(cudaMemcpyAsync(e->page_table, pt.data(), pt.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    e->page_table_host = pt;
     // inv_freq as transformers computes it (modeling_rope_utils.py): default theta^(-2i/d), then the
     // checkpoint's scaling rule; angle and cos/sin in fp32 like LlamaRotaryEmbedding.forward
     const int half = c.head_dim / 2;
@@ -1199,7 +1207,7 @@ void lsk_destroy(lsk_engine* e) {
                   e->hidden, e->qbuf, e->attn_out, e->act, e->tp_buf, e->logits, e->logits_gath, e->logits_full, e->probs_d, e->probs_v, e->samp_scratch, e->cand_val,
                   e->cand_idx, e->gath_val, e->gath_idx, e->ban_val, e->ban_idx, e->rank_val, e->rank_idx,
                   e->d_zero, e->d_prompt, e->state, e->gen_dev, e->attn_part, e->attn_arrive,
-                  e->score_lp, e->score_greedy, e->batch_buf, e->piece_arrive, e->exits_lp, e->exits_greedy,
+                  e->score_lp, e->score_greedy, e->batch_buf, e->piece_arrive, e->view_table, e->exits_lp, e->exits_greedy,
                   e->exits_accept, e->exits_pd, e->exits_pv};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->res_host) cudaFreeHost(e->res_host);
@@ -1693,6 +1701,42 @@ int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer, 
   return LSK_OK;
 }
 
+// Attention pieces of nr packed rows at group rows r .. r + nr - 1, positions pos0 .., first page
+// `page`: maximal runs inside one 128-row chunk, cut to the m_attn rows one prompt-attention launch
+// holds.  chunk_first[c] is the first piece of chunk c.
+static void add_pieces(std::vector<int4>& pieces, std::vector<int>& chunk_first, int r, int nr, int pos0, int page,
+                       int m_attn) {
+  for (int i = 0; i < nr;) {
+    const int row = r + i, chunk = row / kPfTokens;
+    const int len = std::min(std::min(nr - i, (chunk + 1) * kPfTokens - row), m_attn);
+    while ((int)chunk_first.size() <= chunk) chunk_first.push_back((int)pieces.size());
+    pieces.push_back(make_int4(row - chunk * kPfTokens, len, pos0 + i, page));
+    i += len;
+  }
+}
+
+// The 128-row chunks of `rows` packed rows through layers [0, E): ids, row map and pieces on the
+// device at d_ids / d_map / d_pieces, the pieces' host copy in pieces / chunk_first (with its final
+// count), first pages indexing `pages` (nullptr: the engine's page table).  With targets every chunk
+// runs to the end and the score head runs on its max_rows slices (score_lp / score_greedy from row
+// c0 on); without, the chunks are a prompt pass that only writes K/V.
+static int enqueue_packed_chunks(lsk_engine* e, int rows, int E, const int* d_ids, const int2* d_map,
+                                 const int4* d_pieces, const std::vector<int4>& pieces,
+                                 const std::vector<int>& chunk_first, const int* d_tgt, const int* pages) {
+  const int hidden = e->cfg.hidden;
+  for (int ci = 0, c0 = 0; c0 < rows; ++ci, c0 += kPfTokens) {
+    const int m = std::min(rows - c0, kPfTokens);
+    PackedChunk pk{d_ids + c0, d_map + c0, d_pieces + chunk_first[ci], chunk_first[ci + 1] - chunk_first[ci], 0, pages};
+    for (int p = chunk_first[ci]; p < chunk_first[ci + 1]; ++p) pk.max_piece_rows = std::max(pk.max_piece_rows, pieces[p].y);
+    TRY(enqueue_prefill_chunk(e, c0, m, E, d_tgt != nullptr, &pk));
+    if (!d_tgt) continue;
+    for (int r0 = 0; r0 < m; r0 += e->max_rows)
+      TRY(enqueue_score_head(e, e->hidden_p + (size_t)r0 * hidden, std::min(m - r0, e->max_rows), d_tgt + c0 + r0,
+                             c0 + r0));
+  }
+  return LSK_OK;
+}
+
 // Teacher-forced scoring of many sequences on the wgmma prompt pass.  The rows of all sequences
 // (row i of a sequence predicts its id i + 1) are concatenated in input order and cut into 128-row
 // chunks.  A group is a run of sequences whose KV pages fit the pool together: sequence j owns the
@@ -1750,13 +1794,7 @@ int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, i
         up[2 * rows + 2 * (r + i)] = i;
         up[2 * rows + 2 * (r + i) + 1] = page;
       }
-      for (int i = 0; i < nr;) {
-        const int row = r + i, chunk = row / kPfTokens;
-        const int len = std::min(std::min(nr - i, (chunk + 1) * kPfTokens - row), m_attn);
-        while ((int)chunk_first.size() <= chunk) chunk_first.push_back((int)pieces.size());
-        pieces.push_back(make_int4(row - chunk * kPfTokens, len, i, page));
-        i += len;
-      }
+      add_pieces(pieces, chunk_first, r, nr, 0, page, m_attn);
       r += nr;
       page += (nr + kPageTokens - 1) / kPageTokens;
     }
@@ -1768,15 +1806,7 @@ int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, i
     const int* d_tgt = e->batch_buf + rows;
     const int2* d_map = reinterpret_cast<const int2*>(e->batch_buf + 2 * rows);
     const int4* d_pieces = reinterpret_cast<const int4*>(e->batch_buf + 4 * rows);
-    for (int ci = 0, c0 = 0; c0 < rows; ++ci, c0 += kPfTokens) {
-      const int m = std::min(rows - c0, kPfTokens);
-      PackedChunk pk{d_ids + c0, d_map + c0, d_pieces + chunk_first[ci], chunk_first[ci + 1] - chunk_first[ci], 0};
-      for (int p = chunk_first[ci]; p < chunk_first[ci + 1]; ++p) pk.max_piece_rows = std::max(pk.max_piece_rows, pieces[p].y);
-      TRY(enqueue_prefill_chunk(e, c0, m, E, true, &pk));
-      for (int r0 = 0; r0 < m; r0 += e->max_rows)
-        TRY(enqueue_score_head(e, e->hidden_p + (size_t)r0 * c.hidden, std::min(m - r0, e->max_rows), d_tgt + c0 + r0,
-                               c0 + r0));
-    }
+    TRY(enqueue_packed_chunks(e, rows, E, d_ids, d_map, d_pieces, pieces, chunk_first, d_tgt, nullptr));
     if (k == n_seqs) CU(cudaEventRecord(e->ev1, e->stream));
     CU(cudaMemcpyAsync(logprob_out + out_row, e->score_lp, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
     if (greedy_out)
@@ -1785,6 +1815,206 @@ int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, i
     j = k;
   }
   CU(cudaStreamSynchronize(e->stream));
+  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
+  return LSK_OK;
+}
+
+// Teacher-forced scoring of branches that continue shared prefixes, on the wgmma prompt pass.  With
+// s = len(P) - 1 and t = s mod 64, a group (prefixes with their branches, as many as the KV pool and
+// the view table hold) runs in two phases:
+//  * prefix phase: rows P[0 .. s) at positions 0 .. s - 1, packed into 128-row chunks, write K/V only
+//    (the prompt pass: the last layer stops after its QKV GEMM, no head);
+//  * branch phase: rows [P[s]] + B[:-1] at positions s .. s + len(B) - 1 with targets B, packed as in
+//    lsk_score_batch and scored.
+// Every sequence reads and writes keys through its own page-table view in view_table: a prefix's view
+// is its own pages; a branch's view is the prefix's s / 64 full pages, then (t > 0) a page holding
+// slots [0, t) of the prefix's partial page, then the branch's own pages.  The prefix's first branch
+// in the group adopts that partial page in place (its rows write slots >= t only); every further
+// branch gets a private copy of slots [0, t), made by one kv_copy_slots_kernel launch between the
+// phases.  Every row's arithmetic is that of lsk_score_batch on P + B, so the results are bit for bit
+// the same.  A prefix whose branches do not all fit runs again in the next group.
+int lsk_score_prefixed(lsk_engine* e, const int32_t* prefix_ids, const int32_t* prefix_offsets, int32_t n_prefixes,
+                       const int32_t* branch_ids, const int32_t* branch_offsets, const int32_t* branch_prefix,
+                       int32_t n_branches, int32_t exit_layer, float* logprob_out, int32_t* greedy_out) {
+  if (!e || !prefix_ids || !prefix_offsets || !branch_ids || !branch_offsets || !branch_prefix || !logprob_out)
+    return fail(LSK_ERR_INVALID, "null argument");
+  const lsk_config& c = e->cfg;
+  if (c.tp_size > 1)
+    return fail(LSK_ERR_INVALID, "lsk_score_prefixed needs tp_size 1: tensor-parallel scoring is not supported");
+  if (!e->pf_tc)
+    return fail(LSK_ERR_INVALID, "lsk_score_prefixed needs the wgmma prompt pass, which this engine does not have");
+  if (n_prefixes < 1) return fail(LSK_ERR_INVALID, "n_prefixes must be at least 1 (got %d)", n_prefixes);
+  if (n_branches < 1) return fail(LSK_ERR_INVALID, "n_branches must be at least 1 (got %d)", n_branches);
+  if (exit_layer > c.n_layers) return fail(LSK_ERR_INVALID, "exit_layer %d > n_layers %d", exit_layer, c.n_layers);
+  auto check_parts = [&](const char* what, const int32_t* ids, const int32_t* off, int n) -> int {
+    if (off[0] != 0) return fail(LSK_ERR_INVALID, "%s offsets[0] must be 0 (got %d)", what, off[0]);
+    for (int j = 0; j < n; ++j) {
+      if (off[j + 1] <= off[j])
+        return fail(LSK_ERR_INVALID, "%s offsets are not increasing at %s %d (%d, %d): each needs at least 1 id", what,
+                    what, j, off[j], off[j + 1]);
+      for (int i = off[j]; i < off[j + 1]; ++i)
+        if (ids[i] < 0 || ids[i] >= c.vocab) return fail(LSK_ERR_INVALID, "%s %d: token id %d out of range", what, j, ids[i]);
+    }
+    return LSK_OK;
+  };
+  TRY(check_parts("prefix", prefix_ids, prefix_offsets, n_prefixes));
+  TRY(check_parts("branch", branch_ids, branch_offsets, n_branches));
+  auto plen = [&](int p) { return prefix_offsets[p + 1] - prefix_offsets[p]; };
+  auto blen = [&](int b) { return branch_offsets[b + 1] - branch_offsets[b]; };
+  std::vector<std::vector<int>> kids(n_prefixes);   // each prefix's branches, in input order
+  for (int b = 0; b < n_branches; ++b) {
+    const int p = branch_prefix[b];
+    if (p < 0 || p >= n_prefixes)
+      return fail(LSK_ERR_INVALID, "branch %d: prefix index %d is outside [0, %d)", b, p, n_prefixes);
+    if (plen(p) + blen(b) > c.max_ctx)
+      return fail(LSK_ERR_CTX, "branch %d: prefix %d + branch = %d ids exceeds max_ctx %d", b, p, plen(p) + blen(b),
+                  c.max_ctx);
+    kids[p].push_back(b);
+  }
+  for (int p = 0; p < n_prefixes; ++p)
+    if (kids[p].empty()) return fail(LSK_ERR_INVALID, "prefix %d has no branch", p);
+  if (!lsk_weights_complete(e)) return fail(LSK_ERR_STATE, "weights not fully loaded");
+  TRY(alloc_scoring(e, true));
+  if (!e->view_table) {
+    const cudaError_t er = cudaMalloc((void**)&e->view_table, (size_t)e->max_pos * 4);
+    if (er != cudaSuccess) {
+      e->view_table = nullptr;
+      return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
+    }
+  }
+  const int E = exit_layer <= 0 ? c.n_layers : exit_layer;
+  const int m_attn = prompt_attn_rows(c.head_dim, e->group);
+  e->prefilled = false;
+  e->host_len = 0;
+
+  struct Member { int p; std::vector<int> br; };
+  std::vector<Member> grp;                 // the group being formed
+  std::vector<int32_t> up, view;           // the group's upload to batch_buf, its page-table views
+  std::vector<int4> pre_pieces, br_pieces, copies;
+  std::vector<int> pre_first, br_first, pre_view, br_view, br_row;
+  std::vector<float> lp_host;
+  std::vector<int32_t> gr_host;
+  // batch_buf sections start 16-byte aligned (row maps are int2, pieces and copies int4)
+  auto section = [&](size_t n) { const size_t o = up.size(); up.resize(o + (n + 3) / 4 * 4, 0); return o; };
+  auto run_group = [&](bool last) -> int {
+    view.clear(); copies.clear(); pre_pieces.clear(); br_pieces.clear();
+    pre_first.clear(); br_first.clear(); pre_view.clear(); br_view.clear(); br_row.clear();
+    int logical = 0, rp = 0, rb = 0;
+    auto new_page = [&]() { return e->page_table_host[logical++]; };
+    for (const Member& g : grp) {
+      const int s = plen(g.p) - 1, nf = s / kPageTokens, t = s % kPageTokens, pv = (int)view.size();
+      pre_view.push_back(pv);
+      for (int k = 0; k < (s + kPageTokens - 1) / kPageTokens; ++k) view.push_back(new_page());
+      rp += s;
+      for (size_t k = 0; k < g.br.size(); ++k) {
+        const int bv = (int)view.size(), n_view = (s + blen(g.br[k]) + kPageTokens - 1) / kPageTokens;
+        for (int q = 0; q < nf; ++q) { const int page = view[pv + q]; view.push_back(page); }
+        if (t > 0) {
+          const int partial = view[pv + nf];
+          if (k == 0) {
+            view.push_back(partial);
+          } else {
+            const int page = new_page();
+            view.push_back(page);
+            copies.push_back(make_int4(partial, page, t, 0));
+          }
+        }
+        while ((int)view.size() - bv < n_view) view.push_back(new_page());
+        br_view.push_back(bv);
+        br_row.push_back(rb);
+        rb += blen(g.br[k]);
+      }
+    }
+    up.clear();
+    const size_t o_pid = section(rp), o_pmap = section(2 * (size_t)rp);
+    const size_t o_bid = section(rb), o_btgt = section(rb), o_bmap = section(2 * (size_t)rb);
+    for (size_t gi = 0, r = 0, bi = 0; gi < grp.size(); ++gi) {
+      const int32_t* P = prefix_ids + prefix_offsets[grp[gi].p];
+      const int s = plen(grp[gi].p) - 1;
+      for (int i = 0; i < s; ++i) {
+        up[o_pid + r + i] = P[i];
+        up[o_pmap + 2 * (r + i)] = i;
+        up[o_pmap + 2 * (r + i) + 1] = pre_view[gi];
+      }
+      add_pieces(pre_pieces, pre_first, (int)r, s, 0, pre_view[gi], m_attn);
+      r += s;
+      for (int b : grp[gi].br) {
+        const int32_t* B = branch_ids + branch_offsets[b];
+        const int lb = blen(b), r0 = br_row[bi];
+        for (int i = 0; i < lb; ++i) {
+          up[o_bid + r0 + i] = i ? B[i - 1] : P[s];
+          up[o_btgt + r0 + i] = B[i];
+          up[o_bmap + 2 * (r0 + i)] = s + i;
+          up[o_bmap + 2 * (r0 + i) + 1] = br_view[bi];
+        }
+        add_pieces(br_pieces, br_first, r0, lb, s, br_view[bi], m_attn);
+        ++bi;
+      }
+    }
+    pre_first.push_back((int)pre_pieces.size());
+    br_first.push_back((int)br_pieces.size());
+    const size_t o_ppc = section(4 * pre_pieces.size()), o_bpc = section(4 * br_pieces.size());
+    const size_t o_cp = section(4 * copies.size());
+    memcpy(up.data() + o_ppc, pre_pieces.data(), pre_pieces.size() * sizeof(int4));
+    memcpy(up.data() + o_bpc, br_pieces.data(), br_pieces.size() * sizeof(int4));
+    memcpy(up.data() + o_cp, copies.data(), copies.size() * sizeof(int4));
+    // every row owns a pool slot and needs at most 8 ints, so a group that fits the pool fits batch_buf
+    if (up.size() > (size_t)8 * e->max_pos)
+      return fail(LSK_ERR_INVALID, "lsk_score_prefixed: group upload of %zu ints exceeds its buffer", up.size());
+    CU(cudaMemcpyAsync(e->batch_buf, up.data(), up.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    CU(cudaMemcpyAsync(e->view_table, view.data(), view.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    const int* d = e->batch_buf;
+    auto i2 = [&](size_t o) { return reinterpret_cast<const int2*>(d + o); };
+    auto i4 = [&](size_t o) { return reinterpret_cast<const int4*>(d + o); };
+    TRY(enqueue_packed_chunks(e, rp, E, d + o_pid, i2(o_pmap), i4(o_ppc), pre_pieces, pre_first, nullptr,
+                              e->view_table));
+    if (!copies.empty()) {
+      e->cur_class = CLS_MISC;
+      CU(launch(e, kv_copy_slots_kernel, dim3((unsigned)copies.size(), E, 2 * e->kv_heads_l), dim3(128), 0, i4(o_cp),
+                e->kpool, e->vpool, e->pool_layer_elems, e->kv_heads_l, c.head_dim));
+    }
+    TRY(enqueue_packed_chunks(e, rb, E, d + o_bid, i2(o_bmap), i4(o_bpc), br_pieces, br_first, d + o_btgt,
+                              e->view_table));
+    if (last) CU(cudaEventRecord(e->ev1, e->stream));
+    lp_host.resize(rb);
+    gr_host.resize(rb);
+    CU(cudaMemcpyAsync(lp_host.data(), e->score_lp, (size_t)rb * 4, cudaMemcpyDeviceToHost, e->stream));
+    if (greedy_out)
+      CU(cudaMemcpyAsync(gr_host.data(), e->score_greedy, (size_t)rb * 4, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    for (size_t gi = 0, bi = 0; gi < grp.size(); ++gi)
+      for (int b : grp[gi].br) {
+        memcpy(logprob_out + branch_offsets[b], lp_host.data() + br_row[bi], (size_t)blen(b) * 4);
+        if (greedy_out) memcpy(greedy_out + branch_offsets[b], gr_host.data() + br_row[bi], (size_t)blen(b) * 4);
+        ++bi;
+      }
+    grp.clear();
+    return LSK_OK;
+  };
+
+  CU(cudaEventRecord(e->ev0, e->stream));
+  int pages = 0, views = 0;   // pool pages and view entries the group uses
+  for (int p = 0; p < n_prefixes; ++p) {
+    const int s = plen(p) - 1, nf = s / kPageTokens, t = s % kPageTokens, own = (s + kPageTokens - 1) / kPageTokens;
+    bool in_group = false;
+    for (int b : kids[p]) {
+      const int n_view = (s + blen(b) + kPageTokens - 1) / kPageTokens;
+      // the prefix's pages come with its first branch in a group, which adopts the partial page
+      auto need_pages = [&]() { return in_group ? n_view - nf : own + n_view - nf - (t > 0 ? 1 : 0); };
+      auto need_views = [&]() { return in_group ? n_view : own + n_view; };
+      if (pages + need_pages() > e->n_pages || views + need_views() > e->max_pos) {
+        TRY(run_group(false));
+        pages = views = 0;
+        in_group = false;
+      }
+      pages += need_pages();
+      views += need_views();
+      if (!in_group) grp.push_back({p, {}});
+      in_group = true;
+      grp.back().br.push_back(b);
+    }
+  }
+  TRY(run_group(true));
   CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
   return LSK_OK;
 }
@@ -1934,6 +2164,7 @@ int lsk_debug_set_page_table(lsk_engine* e, const int32_t* pages, int32_t n) {
   }
   CU(cudaMemcpyAsync(e->page_table, pages, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
   CU(cudaStreamSynchronize(e->stream));
+  e->page_table_host.assign(pages, pages + n);
   return LSK_OK;
 }
 

@@ -75,6 +75,27 @@ __global__ void embed_tokens_kernel(const __nv_bfloat16* __restrict__ embed, int
             blockDim.x);
 }
 
+// ---------------------------------------------------------------------------------------
+// KV slot copy (prefix-shared scoring): entry blockIdx.x = (src page, dst page, t) copies token
+// slots [0, t) of one (layer blockIdx.y, K or V, kv head) block from the src page to the dst page.
+// The slots of a (page, kv head) block are contiguous rows and are copied slot for slot, so the
+// swizzle inside each row (kv_elem_offset) carries over unchanged.
+// grid (entries, layers, 2 * n_kv_heads)
+// ---------------------------------------------------------------------------------------
+__global__ void kv_copy_slots_kernel(const int4* __restrict__ entries, __nv_bfloat16* __restrict__ kpool,
+                                     __nv_bfloat16* __restrict__ vpool, size_t layer_elems, int n_kv_heads,
+                                     int hd) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int4 en = entries[blockIdx.x];
+  const int head = blockIdx.z >> 1;
+  __nv_bfloat16* pool = ((blockIdx.z & 1) ? vpool : kpool) + (size_t)blockIdx.y * layer_elems;
+  const uint4* src = reinterpret_cast<const uint4*>(pool + kv_elem_offset(hd, en.x, n_kv_heads, head, 0, 0));
+  uint4* dst = reinterpret_cast<uint4*>(pool + kv_elem_offset(hd, en.y, n_kv_heads, head, 0, 0));
+  const int n = en.z * hd / 8;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
+}
+
 // Candidate arg-max reduction for token row `row` (warp-wide, fixed order).
 __device__ __forceinline__ int reduce_candidates(const float* __restrict__ val,
                                                  const int* __restrict__ idx, int n_cand,

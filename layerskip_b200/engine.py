@@ -250,6 +250,36 @@ class Engine:
             out.append((logprobs[r0:r0 + len(s) - 1], greedy[r0:r0 + len(s) - 1]))
         return out
 
+    def score_prefixed(self, prefixes: Sequence[Sequence[int]], branches: Sequence[Tuple[int, Sequence[int]]],
+                       exit_layer: int = -1) -> List[Tuple[torch.Tensor, torch.Tensor]]:
+        """Score continuations that share contexts: `branches` holds (prefix index, ids B) pairs, each
+        scoring prefixes[index] + B.  Each prefix's own rows run once (per KV group) and only write
+        keys and values; the branches' rows are packed into shared 128-token chunks on top of them.
+        Returns one (logprobs float32[len(B)], greedy int64[len(B)]) per branch, in order: entry i is
+        the log-probability of B[i] after P + B[:i] and the arg-max token there, bit-identical to
+        entries len(P)-1 .. of `score_batch([P + B])`.  Every prefix and branch needs at least one
+        id, every prefix at least one branch.  Needs an engine with the prompt pass."""
+        prefixes = [[int(t) for t in p] for p in prefixes]
+        branches = [(int(p), [int(t) for t in b]) for p, b in branches]
+        p_off, b_off = [0], [0]
+        for p in prefixes:
+            p_off.append(p_off[-1] + len(p))
+        for _, b in branches:
+            b_off.append(b_off[-1] + len(b))
+        p_ids = [t for p in prefixes for t in p]
+        b_ids = [t for _, b in branches for t in b]
+        i32 = lambda v: (C.c_int32 * max(len(v), 1))(*v)   # noqa: E731
+        rows = max(b_off[-1], 1)
+        lp = (C.c_float * rows)()
+        gr = (C.c_int32 * rows)()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_score_prefixed(self._h, i32(p_ids), i32(p_off), len(prefixes), i32(b_ids),
+                                                    i32(b_off), i32([p for p, _ in branches]), len(branches),
+                                                    int(exit_layer), lp, gr))
+        logprobs = torch.frombuffer(lp, dtype=torch.float32).clone()
+        greedy = torch.frombuffer(gr, dtype=torch.int32).clone().to(torch.int64)
+        return [(logprobs[b_off[j]:b_off[j + 1]], greedy[b_off[j]:b_off[j + 1]]) for j in range(len(branches))]
+
     def score_exits(self, ids: Sequence[int], exits: Sequence[int], sampling: Optional[Dict] = None
                     ) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
         """`score(ids, E)` at every exit E of `exits` (strictly increasing, in [1, layers]) in one
@@ -312,11 +342,44 @@ class Engine:
         logprobs, greedy = self.score(self._loglikelihood_ids(context, continuation), exit_layer)
         return self._continuation_score(logprobs, greedy, continuation)
 
+    @staticmethod
+    def _prefix_plan(seqs: List[List[int]], conts: List[List[int]]):
+        """Requests grouped by their (cut) context: a context that two or more requests share becomes
+        one prefix with their continuations as branches; every other request becomes a branch of a
+        prefix of its own first id.  Returns (prefixes, branches, use), `use` telling whether
+        `score_prefixed` needs fewer 128-row chunks than `score_batch` of the joined sequences."""
+        ctxs = [tuple(s[:len(s) - len(k)]) for s, k in zip(seqs, conts)]
+        count: Dict[tuple, int] = {}
+        for c in ctxs:
+            count[c] = count.get(c, 0) + 1
+        prefixes: List[List[int]] = []
+        branches: List[Tuple[int, List[int]]] = []
+        index: Dict[tuple, int] = {}
+        for s, k, c in zip(seqs, conts, ctxs):
+            if count[c] >= 2:
+                if c not in index:
+                    index[c] = len(prefixes)
+                    prefixes.append(list(c))
+                branches.append((index[c], k))
+            else:
+                prefixes.append(s[:1])
+                branches.append((len(prefixes) - 1, s[1:]))
+        chunks = lambda rows: (rows + 127) // 128    # noqa: E731
+        prefix_rows = sum(len(p) - 1 for p in prefixes)
+        branch_rows = sum(len(b) for _, b in branches)
+        batch_rows = sum(len(s) - 1 for s in seqs)
+        return prefixes, branches, chunks(prefix_rows) + chunks(branch_rows) < chunks(batch_rows)
+
     def loglikelihood_batch(self, requests: Sequence[Tuple[Sequence[int], Sequence[int]]],
                             exit_layer: int = -1) -> List[Tuple[float, bool]]:
         """`loglikelihood` of every (context, continuation) request, in order, with one
         `score_batch` call for all of them (every request is validated before any is scored).  On an
         engine without the wgmma prompt pass it calls `loglikelihood` once per request.
+
+        Requests that share a context (after the left cut), such as the choices of a multiple-choice
+        question, are scored with one `score_prefixed` call instead when that packs into fewer
+        128-row chunks: the shared context then runs once rather than once per request.  Both calls
+        give the same bits, so the choice changes only the time taken.
 
         Caveat: a request whose joined ids number at most max_rows + 1 is scored here on the wgmma
         route, while `loglikelihood` scores it on the decode route.  The two then agree within the
@@ -327,7 +390,11 @@ class Engine:
             return []
         if not (self.prefill_tc and self.arch.hidden % 64 == 0):
             return [self.loglikelihood(ctx, cont, exit_layer) for ctx, cont in reqs]
-        scored = self.score_batch(seqs, exit_layer)
+        prefixes, branches, use_prefixed = self._prefix_plan(seqs, [cont for _, cont in reqs])
+        if use_prefixed:
+            scored = self.score_prefixed(prefixes, branches, exit_layer)
+        else:
+            scored = self.score_batch(seqs, exit_layer)
         return [self._continuation_score(lp, gr, cont) for (lp, gr), (_, cont) in zip(scored, reqs)]
 
     # ------------------------------------------------------------------ introspection

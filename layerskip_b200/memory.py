@@ -20,7 +20,7 @@ SM_COUNT = 132                      # H100 SXM: one arg-max candidate slot per S
 def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling: bool = False,
                 keep_logits: bool = False, lm_head_tc: bool = False, prefill_tc: bool = True,
                 scoring: bool = False, batch_scoring: bool = False, score_exits: int = 0,
-                score_exits_sampled: bool = False) -> Dict[str, int]:
+                score_exits_sampled: bool = False, prefix_scoring: bool = False) -> Dict[str, int]:
     """Bytes the engine allocates on ONE rank.  Keys: weights, embed, lm_head, kv_pool, scratch,
     total (+ weights_source_peak: the largest single tensor staged on the GPU while loading).
     `scoring` adds what the first `lsk_score` call allocates: the logits rows (unless already
@@ -31,9 +31,12 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
     = k adds what the first `lsk_score_exits` call with k exits allocates: the logits rows (unless
     already there) and k floats + k ints per position; `score_exits_sampled` adds, for the k - 1
     draft exits, one float per position and the warped draft rows of a chunk (128 rows with the
-    prompt pass, 16 without), plus 16 warped full-depth rows."""
+    prompt pass, 16 without), plus 16 warped full-depth rows.  `prefix_scoring` adds what the first
+    `lsk_score_prefixed` call allocates: what `batch_scoring` adds, and one int per position for the
+    table of page-table views."""
     h, L = arch.hidden, arch.layers
-    batch_scoring = batch_scoring and prefill_tc and h % 64 == 0
+    prefix_scoring = prefix_scoring and prefill_tc and h % 64 == 0
+    batch_scoring = (batch_scoring or prefix_scoring) and prefill_tc and h % 64 == 0
     scoring = scoring or batch_scoring
     q_l = arch.heads // tp_size * arch.head_dim
     kv_l = arch.kv_heads // tp_size * arch.head_dim
@@ -80,6 +83,8 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
         scratch += 2 * max_pos * 4                          # per-position log-probabilities + arg-max ids
     if batch_scoring:
         scratch += 8 * max_pos * 4 + 128 * kvh_l * 4        # packed group arrays + piece arrival counters
+    if prefix_scoring:
+        scratch += max_pos * 4                              # page-table views of a group
     if sampling:
         scratch += (2 * MAX_ROWS + 1) * arch.vocab * 4
         if tp_size > 1:
