@@ -149,6 +149,21 @@ int lsk_prefill(lsk_engine* e, const int32_t* ids, int32_t n);
  * d_req == 0 is the reference's tail round.  Blocks until the round's result is on the host. */
 int lsk_round(lsk_engine* e, int32_t d_req, lsk_round_out* out);
 
+/* A round that stops drafting when the early-exit head is unsure (Hugging Face assisted
+ * generation's assistant_confidence_threshold).  The confidence of draft i is the probability of
+ * the token it chose under the distribution it chose from: softmax(logits)[arg-max] at temperature
+ * 1 when greedy, the warped draft row's probability of the drawn token when sampling (both after
+ * the n-gram ban, if any).  n_drafted = 1 + the first i whose draft is an EOS or has confidence
+ * < min_confidence, else d_max; the stopping draft is kept.  The draft steps after it do not run
+ * (graph mode; LSK_FLAG_NO_GRAPH runs them and ignores their results).
+ * The result, and the state left behind, are bit-identical to lsk_round(e, n_drafted, out) from
+ * the same state; min_confidence == 0 gives lsk_round(e, d_max, out).
+ * draft_conf_out (host, may be NULL, LSK_MAX_SPEC entries) receives confidences 0 .. n_drafted-1.
+ * Same preconditions and errors as lsk_round with d_max for d_req; also LSK_ERR_INVALID for
+ * min_confidence outside [0, 1] or NaN, and for tp_size > 1. */
+int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_round_out* out,
+                       float* draft_conf_out);
+
 /* One autoregressive step on the same engine (autoregressive_generator.py:44-67): all layers, or
  * layers < E when the generation's exit_layer > 0.  Returns the chosen token; the caller decides
  * about EOS exactly as the reference does (:66-67). */

@@ -94,6 +94,8 @@ SIGNATURES = {
     "lsk_begin": (C.c_int, [C.c_void_p, C.POINTER(lsk_generation)]),
     "lsk_prefill": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
     "lsk_round": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(lsk_round_out)]),
+    "lsk_round_adaptive": (C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.POINTER(lsk_round_out),
+                                     C.POINTER(C.c_float)]),
     "lsk_ar_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "lsk_score": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32,
                             C.POINTER(C.c_float), C.POINTER(C.c_int32)]),

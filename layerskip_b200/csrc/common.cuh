@@ -140,6 +140,11 @@ struct DevState {
   int n_prompt;               // prompt length: hist[n_prompt + n_out] is where the next emitted token goes
   int tok[kMaxRows + 1];
   int verified[kMaxRows + 1];
+  // adaptive rounds (lsk_round_adaptive): the threshold the host set for this round, the draft
+  // confidences, and d_stop = the number of drafts the round keeps
+  float min_conf;
+  float conf[kMaxRows];
+  int d_stop;
 };
 
 }  // namespace lsk

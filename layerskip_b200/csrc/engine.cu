@@ -98,6 +98,8 @@ struct lsk_engine {
   int n_pages = 0, max_pos = 0, n_splits = 0;
   int max_rows = kMaxRows;             // token rows one step can carry (8 when 16 do not fit)
   bool use_pdl = true, use_graph = true, keep_logits = false;
+  bool pdl_break = false;              // launch the next kernel without the PDL attribute (graph conditional boundary)
+  bool adaptive = false;               // enqueueing an adaptive round: draft heads materialise their logits
 
   std::vector<LayerWeights> layers;
   __nv_bfloat16* embed = nullptr;      // [vocab, hidden] natural (replicated)
@@ -177,6 +179,8 @@ struct lsk_engine {
   int cur_n_cand = 0;
 
   cudaStream_t stream = nullptr;
+  cudaStream_t body_stream = nullptr;  // captures the bodies of an adaptive round's conditional nodes
+  ConfScratch* conf_scratch = nullptr; // draft_confidence_kernel's partials and arrival counter
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::map<long long, cudaGraphExec_t> graphs;
   ncclComm_t comm = nullptr;
@@ -228,6 +232,8 @@ static auto stream_op(lsk_engine* e, int cls, F enqueue) -> decltype(enqueue()) 
 }
 
 // Kernel launch: programmatic dependent launch attribute on every kernel, class = e->cur_class.
+// A programmatic edge cannot cross into or out of a graph conditional body: the first kernel of a
+// body and the first kernel after one are launched without it (e->pdl_break).
 template <typename... KArgs, typename... Args>
 static cudaError_t launch(lsk_engine* e, void (*kern)(KArgs...), dim3 grid, dim3 block,
                           size_t smem, Args... args) {
@@ -240,7 +246,8 @@ static cudaError_t launch(lsk_engine* e, void (*kern)(KArgs...), dim3 grid, dim3
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  cfg.numAttrs = e->use_pdl ? 1 : 0;
+  cfg.numAttrs = (e->use_pdl && !e->pdl_break) ? 1 : 0;
+  e->pdl_break = false;
   return stream_op(e, e->cur_class, [&]() { return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...); });
 }
 
@@ -757,10 +764,10 @@ static int emit_finalize(lsk_engine* e, int slot, float* dst_row) {
 }
 // token history (prompt ids + emitted tokens) is kept on the device only when the n-gram ban needs it
 static int* hist_ptr(lsk_engine* e) { return e->gen.no_repeat_ngram_size > 0 ? e->d_prompt : nullptr; }
-static int emit_accept(lsk_engine* e, int d_spec) {
+static int emit_accept(lsk_engine* e, int d_spec, const int* d_stop) {
   e->cur_class = CLS_MISC;
   CU(launch(e, accept_greedy_kernel, dim3(1), dim3(256), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e), d_spec,
-            e->state, (const GenParams*)e->gen_dev, e->res_dev, 0, hist_ptr(e)));
+            e->state, (const GenParams*)e->gen_dev, e->res_dev, 0, hist_ptr(e), d_stop));
   return LSK_OK;
 }
 static int emit_ar_commit(lsk_engine* e) {
@@ -797,7 +804,7 @@ static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0) {
   const bool ban = e->gen.no_repeat_ngram_size > 0;
   e->cur_class = CLS_LMHEAD;
   const float* x = e->hidden + (size_t)row0 * c.hidden;
-  float* logits = (e->keep_logits || e->gen.sample || ban) ? e->logits : nullptr;
+  float* logits = (e->keep_logits || e->gen.sample || ban || e->adaptive) ? e->logits : nullptr;
   if (e->lm_tc) {
     if (!(e->ablate & (1u << CLS_LMHEAD))) {
       LmHeadTcArgs t{};
@@ -853,8 +860,48 @@ static int n_cand(lsk_engine* e) { return e->cfg.tp_size > 1 ? e->cfg.tp_size : 
 // ---------------------------------------------------------------------------------------------
 // round / AR-step command streams
 // ---------------------------------------------------------------------------------------------
-static int enqueue_round(lsk_engine* e, int E, int d) {
+// Draft step i after its layers: the shared head on row i; its token becomes tok[i+1] and is
+// embedded into row i+1.
+static int enqueue_draft_token(lsk_engine* e, int i) {
   const lsk_config& c = e->cfg;
+  TRY(enqueue_lm_head(e, i, 1, i));
+  e->cur_class = CLS_MISC;
+  if (!e->gen.sample) {
+    TRY(emit_finalize(e, 1 + i, e->hidden + (size_t)(i + 1) * c.hidden));
+  } else {
+    // decode_next_token sampling branch (llama_model_utils.py:123-131): keep the warped
+    // distribution of draft i (needed by the rejection test), draw tok[i+1], embed it.
+    CU(launch(e, warp_and_sample_kernel, dim3(1), dim3(kSampleThreads), 0, samp_logits(e),
+              samp_ld(e), c.vocab, (const GenParams*)e->gen_dev, (const DevState*)e->state,
+              e->probs_d + (size_t)i * c.vocab, &e->state->tok[1 + i], (int)RNG_DRAFT, i));
+    CU(launch(e, embed_tokens_kernel, dim3(1), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
+              (const int*)&e->state->tok[1 + i], e->hidden + (size_t)(i + 1) * c.hidden, c.hidden));
+  }
+  return LSK_OK;
+}
+
+// Verify after the draft rows: layers >= E see [exit rows of the draft steps ; the last draft's row]
+// = rows 0..d (:363-383), then the head and the accept / commit.  d_stop: see accept_commit.
+static int enqueue_verify(lsk_engine* e, int E, int d, const int* d_stop) {
+  const lsk_config& c = e->cfg;
+  const int* len = &e->state->len;
+  for (int l = E; l < c.n_layers; ++l) TRY(enqueue_layer(e, l, 0, d + 1, len, 0));
+  TRY(enqueue_lm_head(e, 0, d + 1, 0));
+  e->cur_class = CLS_MISC;
+  if (!e->gen.sample) {
+    TRY(emit_accept(e, d, d_stop));
+  } else {
+    CU(launch(e, warp_and_sample_kernel, dim3(d + 1), dim3(kSampleThreads), 0, samp_logits(e),
+              samp_ld(e), c.vocab, (const GenParams*)e->gen_dev, (const DevState*)e->state,
+              e->probs_v, &e->state->verified[0], (int)RNG_VERIFY, 0));
+    CU(launch(e, accept_sample_kernel, dim3(1), dim3(kSampleThreads), 0, (const float*)e->probs_d,
+              (const float*)e->probs_v, c.vocab, d, e->state, (const GenParams*)e->gen_dev, e->res_dev,
+              e->samp_scratch, 0, hist_ptr(e), d_stop));
+  }
+  return LSK_OK;
+}
+
+static int enqueue_round(lsk_engine* e, int E, int d) {
   const int* len = &e->state->len;
   // row 0 <- embedding of the pending token (self_speculation_generator.py:122, input_ids)
   TRY(emit_embed(e, &e->state->tok[0], e->hidden, 1));
@@ -862,38 +909,91 @@ static int enqueue_round(lsk_engine* e, int E, int d) {
   // head; its arg-max becomes tok[i+1] and is embedded into row i+1.
   for (int i = 0; i < d; ++i) {
     for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, i, 1, len, i));
-    TRY(enqueue_lm_head(e, i, 1, i));
-    e->cur_class = CLS_MISC;
-    if (!e->gen.sample) {
-      TRY(emit_finalize(e, 1 + i, e->hidden + (size_t)(i + 1) * c.hidden));
-    } else {
-      // decode_next_token sampling branch (llama_model_utils.py:123-131): keep the warped
-      // distribution of draft i (needed by the rejection test), draw tok[i+1], embed it.
-      CU(launch(e, warp_and_sample_kernel, dim3(1), dim3(kSampleThreads), 0, samp_logits(e),
-                samp_ld(e), c.vocab, (const GenParams*)e->gen_dev, (const DevState*)e->state,
-                e->probs_d + (size_t)i * c.vocab, &e->state->tok[1 + i], (int)RNG_DRAFT, i));
-      CU(launch(e, embed_tokens_kernel, dim3(1), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
-                (const int*)&e->state->tok[1 + i], e->hidden + (size_t)(i + 1) * c.hidden, c.hidden));
-    }
+    TRY(enqueue_draft_token(e, i));
   }
   // verify (:164-174 -> llama_model_utils.py:280-391): the last drafted token has not been
   // through layers < E yet (:350-362) ...
   for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, d, 1, len, d));
-  // ... then layers >= E see [exit rows of the draft steps ; that row] = rows 0..d (:363-383)
-  for (int l = E; l < c.n_layers; ++l) TRY(enqueue_layer(e, l, 0, d + 1, len, 0));
-  TRY(enqueue_lm_head(e, 0, d + 1, 0));
+  // ... then layers >= E on rows 0..d
+  return enqueue_verify(e, E, d, nullptr);
+}
+
+// Confidence and stop rule of draft step j (draft_confidence_kernel).
+static int emit_draft_confidence(lsk_engine* e, int j, int d, cudaGraphConditionalHandle next, bool has_next) {
+  const lsk_config& c = e->cfg;
   e->cur_class = CLS_MISC;
-  if (!e->gen.sample) {
-    TRY(emit_accept(e, d));
-  } else {
-    CU(launch(e, warp_and_sample_kernel, dim3(d + 1), dim3(kSampleThreads), 0, samp_logits(e),
-              samp_ld(e), c.vocab, (const GenParams*)e->gen_dev, (const DevState*)e->state,
-              e->probs_v, &e->state->verified[0], (int)RNG_VERIFY, 0));
-    CU(launch(e, accept_sample_kernel, dim3(1), dim3(kSampleThreads), 0, (const float*)e->probs_d,
-              (const float*)e->probs_v, c.vocab, d, e->state, (const GenParams*)e->gen_dev, e->res_dev,
-              e->samp_scratch, 0, hist_ptr(e)));
-  }
+  const int grid = std::min(kConfMaxCtas, (c.vocab + kConfCols - 1) / kConfCols);
+  const float* logits = e->gen.sample ? nullptr : (const float*)e->logits;
+  const float* probs = e->gen.sample ? (const float*)e->probs_d + (size_t)j * c.vocab : nullptr;
+  CU(launch(e, draft_confidence_kernel, dim3(grid), dim3(kConfThreads), 0, logits, probs, c.vocab, e->state,
+            (const GenParams*)e->gen_dev, e->conf_scratch, j, d, e->hidden, c.hidden, next, (int)has_next));
   return LSK_OK;
+}
+
+// `body` enqueued as the body of a graph IF node on `cond` while e->stream is being captured (the
+// body is captured on e->body_stream), or launched directly in eager mode.
+template <typename F>
+static int enqueue_if(lsk_engine* e, cudaGraphConditionalHandle cond, F body) {
+  if (!e->use_graph) return body();
+  cudaStreamCaptureStatus cs;
+  cudaGraph_t graph = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t n_deps = 0;
+  CU(cudaStreamGetCaptureInfo(e->stream, &cs, nullptr, &graph, &deps, &n_deps));
+  if (cs != cudaStreamCaptureStatusActive) return fail(LSK_ERR_CUDA, "adaptive round: stream is not capturing");
+  cudaGraphNodeParams p = {};
+  p.type = cudaGraphNodeTypeConditional;
+  p.conditional.handle = cond;
+  p.conditional.type = cudaGraphCondTypeIf;
+  p.conditional.size = 1;
+  cudaGraphNode_t node;
+  CU(cudaGraphAddNode(&node, graph, deps, n_deps, &p));
+  CU(cudaStreamBeginCaptureToGraph(e->body_stream, p.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                   cudaStreamCaptureModeRelaxed));
+  cudaStream_t outer = e->stream;
+  e->stream = e->body_stream;
+  e->pdl_break = true;
+  const int st = body();
+  e->stream = outer;
+  cudaGraph_t body_graph = nullptr;
+  const cudaError_t ce = cudaStreamEndCapture(e->body_stream, &body_graph);
+  if (st != LSK_OK) return st;
+  if (ce != cudaSuccess) return fail(LSK_ERR_CUDA, "conditional body capture failed: %s", cudaGetErrorString(ce));
+  CU(cudaStreamUpdateCaptureDependencies(e->stream, &node, 1, cudaStreamSetCaptureDependencies));
+  e->pdl_break = true;
+  return LSK_OK;
+}
+
+// Adaptive round (lsk_round_adaptive): the rows of enqueue_round(E, d), but draft step j >= 1 runs
+// only while no earlier draft has stopped the round (draft_confidence_kernel).  Each conditional
+// body j holds step j's head, token and stop test, then the layers < E of row j + 1, the token
+// step j chose: both run iff j < d_stop.  For j = d - 1 those layers are the verify's row d.
+// Step 0 and the layers of row 1 always run (d_stop >= 1).  Layers >= E run on rows 0..d whatever
+// d_stop is; rows past d_stop are finite (zeroed by step 0) and causally invisible to the kept rows.
+static int enqueue_round_adaptive(lsk_engine* e, int E, int d) {
+  const int* len = &e->state->len;
+  std::vector<cudaGraphConditionalHandle> cond(d, 0);
+  if (e->use_graph) {
+    cudaStreamCaptureStatus cs;
+    cudaGraph_t graph = nullptr;
+    CU(cudaStreamGetCaptureInfo(e->stream, &cs, nullptr, &graph, nullptr, nullptr));
+    for (int j = 1; j < d; ++j) CU(cudaGraphConditionalHandleCreate(&cond[j], graph, 0, cudaGraphCondAssignDefault));
+  }
+  const bool graph = e->use_graph;
+  TRY(emit_embed(e, &e->state->tok[0], e->hidden, 1));
+  for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, 0, 1, len, 0));
+  TRY(enqueue_draft_token(e, 0));
+  TRY(emit_draft_confidence(e, 0, d, graph && d > 1 ? cond[1] : 0, graph && d > 1));
+  for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, 1, 1, len, 1));
+  for (int j = 1; j < d; ++j) {
+    TRY(enqueue_if(e, cond[j], [&]() -> int {
+      TRY(enqueue_draft_token(e, j));
+      TRY(emit_draft_confidence(e, j, d, graph && j + 1 < d ? cond[j + 1] : 0, graph && j + 1 < d));
+      for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, j + 1, 1, len, j + 1));
+      return LSK_OK;
+    }));
+  }
+  return enqueue_verify(e, E, d, &e->state->d_stop);
 }
 
 static int enqueue_ar(lsk_engine* e, int n_layers_run) {
@@ -1214,6 +1314,8 @@ void lsk_destroy(lsk_engine* e) {
   if (e->ev0) cudaEventDestroy(e->ev0);
   if (e->ev1) cudaEventDestroy(e->ev1);
   if (e->stream) cudaStreamDestroy(e->stream);
+  if (e->body_stream) cudaStreamDestroy(e->body_stream);
+  if (e->conf_scratch) cudaFree(e->conf_scratch);
   cudaGetLastError();   // a half-built engine may have left a sticky-free error behind
   delete e;
 }
@@ -1537,6 +1639,48 @@ int lsk_round(lsk_engine* e, int32_t d_req, lsk_round_out* out) {
   TRY(run_cached(e, key, [&]() { return enqueue_round(e, E, d_req); }));
   TRY(peer_check(e));
   copy_result(e, out);
+  e->host_len = out->kv_len;
+  return LSK_OK;
+}
+
+int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_round_out* out,
+                       float* draft_conf_out) {
+  if (!e || !out) return fail(LSK_ERR_INVALID, "null argument");
+  if (!(min_confidence >= 0.f && min_confidence <= 1.f))
+    return fail(LSK_ERR_INVALID, "min_confidence %g outside [0, 1]", (double)min_confidence);
+  if (e->cfg.tp_size > 1) return fail(LSK_ERR_INVALID, "lsk_round_adaptive needs tp_size == 1");
+  if (!e->prefilled) return fail(LSK_ERR_STATE, "lsk_prefill must precede lsk_round_adaptive");
+  if (d_max < 0 || d_max + 1 > e->max_rows) return fail(LSK_ERR_INVALID, "d_max %d out of [0,%d]", d_max, e->max_rows - 1);
+  const int E = e->gen.exit_layer;
+  if (E < 1 || E > e->cfg.n_layers) return fail(LSK_ERR_INVALID, "self-speculation needs 1 <= exit_layer <= n_layers (got %d)", E);
+  if (e->host_len + d_max + 2 > e->max_pos) return fail(LSK_ERR_CTX, "context %d + %d exceeds max_ctx", e->host_len, d_max + 1);
+  if (d_max == 0) return lsk_round(e, 0, out);      // no draft to stop: the reference's tail round
+  if (e->use_graph && !e->body_stream) {
+    int drv = 0;
+    CU(cudaDriverGetVersion(&drv));
+    if (drv < 12040) return fail(LSK_ERR_CUDA, "adaptive rounds need CUDA graph conditional nodes (driver >= 12.4, found %d)", drv);
+    CU(cudaStreamCreateWithFlags(&e->body_stream, cudaStreamNonBlocking));
+  }
+  if (!e->conf_scratch) {
+    CU(cudaMalloc((void**)&e->conf_scratch, sizeof(ConfScratch)));
+    CU(cudaMemsetAsync(e->conf_scratch, 0, sizeof(ConfScratch), e->stream));
+  }
+  if (!e->logits) {                       // greedy drafts materialise their logits row
+    cudaError_t er = cudaMalloc((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4);
+    if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
+  }
+  // the threshold is read from device memory: one graph per round shape serves every threshold
+  CU(cudaMemcpyAsync(&e->state->min_conf, &min_confidence, sizeof(float), cudaMemcpyHostToDevice, e->stream));
+  const long long key = ((long long)E << 20) | ((long long)d_max << 8) | (e->gen.sample ? 4 : 0) | 8 | 1 |
+                        ((long long)e->gen.no_repeat_ngram_size << 32);
+  e->adaptive = true;
+  const int st = run_cached(e, key, [&]() { return enqueue_round_adaptive(e, E, d_max); });
+  e->adaptive = false;
+  e->pdl_break = false;
+  TRY(st);
+  copy_result(e, out);
+  if (draft_conf_out)
+    for (int i = 0; i < out->n_drafted; ++i) draft_conf_out[i] = e->res_host->conf[i];
   e->host_len = out->kv_len;
   return LSK_OK;
 }
@@ -2680,7 +2824,7 @@ int lsk_test_accept_sample(const float* p_draft, const float* p_verify, int32_t 
   CU(cudaMemset(res_dev, 0, (size_t)n_steps * sizeof(RoundResult)));
   for (int s = 0; s < n_steps; ++s)
     accept_sample_kernel<<<1, kSampleThreads>>>(p_draft, p_verify, vocab, d, st_dev + s, gp_dev, res_dev + s,
-                                                residual, s + 1, (int*)nullptr);
+                                                residual, s + 1, (int*)nullptr, (const int*)nullptr);
   CU(cudaGetLastError());
   CU(cudaDeviceSynchronize());
   std::vector<RoundResult> res((size_t)n_steps);

@@ -163,6 +163,7 @@ struct RoundResult {
   int draft_ids[kMaxRows];
   int emitted_ids[kMaxRows];
   int verified_ids[kMaxRows];
+  float conf[kMaxRows];   // adaptive rounds: confidence of each kept draft
   int seq;   // written last: host-visible completion stamp
 };
 
@@ -179,13 +180,19 @@ __device__ __forceinline__ bool is_eos(const GenParams& gp, int tok) {
 // not exist": d_actual = index of first EOS + 1.  Rows past d_actual were computed but, the
 // attention being causal, cannot influence rows <= d_actual; their KV entries lie beyond the
 // committed length and are overwritten later.
+// An adaptive round (d_stop != nullptr) drafted *d_stop tokens of the d it has rows for: drafts
+// after the first EOS or the first unsure token do not exist either, and their confidences go out.
 // thread-0 part of the greedy accept: compares drafts with the verifier's arg-maxes, commits.
 __device__ __forceinline__ void accept_commit(const int* s_ver, int d, DevState* __restrict__ st,
                                               const GenParams& g, RoundResult* __restrict__ res,
-                                              int seq, int* __restrict__ hist = nullptr) {
-  int d_act = d;
-  for (int i = 0; i < d; ++i)
+                                              int seq, int* __restrict__ hist = nullptr,
+                                              const int* __restrict__ d_stop = nullptr) {
+  const int d_lim = d_stop != nullptr ? *d_stop : d;
+  int d_act = d_lim;
+  for (int i = 0; i < d_lim; ++i)
     if (is_eos(g, st->tok[1 + i])) { d_act = i + 1; break; }
+  if (d_stop != nullptr)
+    for (int i = 0; i < d_act; ++i) res->conf[i] = st->conf[i];
   int n = 0;
   while (n < d_act && st->tok[1 + n] == s_ver[n]) ++n;
   res->n_drafted = d_act;
@@ -210,7 +217,8 @@ __device__ __forceinline__ void accept_commit(const int* s_ver, int d, DevState*
 __global__ void accept_greedy_kernel(const float* __restrict__ cand_val,
                                      const int* __restrict__ cand_idx, int n_cand, int d,
                                      DevState* __restrict__ st, const GenParams* __restrict__ gp,
-                                     RoundResult* __restrict__ res, int seq, int* __restrict__ hist) {
+                                     RoundResult* __restrict__ res, int seq, int* __restrict__ hist,
+                                     const int* __restrict__ d_stop) {
   __shared__ int s_ver[kMaxRows];
   pdl_launch_dependents();
   pdl_wait();
@@ -220,7 +228,7 @@ __global__ void accept_greedy_kernel(const float* __restrict__ cand_val,
     if (lane == 0) s_ver[row] = tok;
   }
   __syncthreads();
-  if (threadIdx.x == 0) accept_commit(s_ver, d, st, *gp, res, seq, hist);
+  if (threadIdx.x == 0) accept_commit(s_ver, d, st, *gp, res, seq, hist, d_stop);
 }
 
 // Autoregressive commit (autoregressive_generator.py:62-76): token = argmax(row 0).

@@ -352,7 +352,7 @@ __global__ void __launch_bounds__(kSampleThreads)
 accept_sample_kernel(const float* __restrict__ p_draft, const float* __restrict__ p_verify, int V,
                      int d, DevState* __restrict__ st, const GenParams* __restrict__ gpp,
                      RoundResult* __restrict__ res, float* __restrict__ scratch, int seq,
-                     int* __restrict__ hist) {
+                     int* __restrict__ hist, const int* __restrict__ d_stop) {
   __shared__ float red[96 + 32];
   __shared__ int s_pick;
   __shared__ int s_n, s_dact, s_reject;
@@ -360,9 +360,13 @@ accept_sample_kernel(const float* __restrict__ p_draft, const float* __restrict_
   pdl_wait();
   const GenParams gp = *gpp;
   if (threadIdx.x == 0) {
-    int d_act = d;
-    for (int i = 0; i < d; ++i)
+    // adaptive rounds: only the first *d_stop drafts exist (accept_commit)
+    const int d_lim = d_stop != nullptr ? *d_stop : d;
+    int d_act = d_lim;
+    for (int i = 0; i < d_lim; ++i)
       if (is_eos(gp, st->tok[1 + i])) { d_act = i + 1; break; }
+    if (d_stop != nullptr)
+      for (int i = 0; i < d_act; ++i) res->conf[i] = st->conf[i];
     int n = 0, reject = -1;
     for (int i = 0; i < d_act; ++i) {
       const int t = st->tok[1 + i];
@@ -426,6 +430,91 @@ __global__ void ar_commit_sampled_kernel(DevState* __restrict__ st, RoundResult*
     __threadfence_system();
     *reinterpret_cast<volatile int*>(&res->seq) = seq;
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Confidence-threshold drafting (lsk_round_adaptive).  After draft step j has chosen tok[1 + j]:
+//   conf[j] = the probability of that token under the distribution it was chosen from:
+//             greedy   softmax(logits row)[arg-max] = 1 / sum_v exp(l_v - max_v l_v)  (T = 1, after the
+//                      n-gram ban when there is one), a log-sum-exp over the CTAs' column slices;
+//             sampling probs[tok], the warped row warp_and_sample_kernel drew from.
+//   The round stops after draft j (d_stop = j + 1) when it is an EOS, when conf[j] < min_conf, or
+//   when j + 1 == d_max; otherwise d_stop = d_max until a later step stops it.  `next` is the graph
+//   conditional that runs step j + 1: set to 1 to go on (its default at every launch is 0).
+// Step 0 also zeroes hidden rows 2 .. d_max: only later draft steps write them, and the verify runs
+// layers >= E on every row, so a row the round skips must hold finite values (0 x NaN in P.V would
+// reach the kept rows).  Causality keeps those rows out of the kept ones.
+// The slices' (max, sum) partials are merged in CTA order by the last CTA to arrive, so the result
+// does not depend on timing; it resets the arrival counter for the next launch.
+// ---------------------------------------------------------------------------------------------
+constexpr int kConfThreads = 512;
+constexpr int kConfMaxCtas = 64;
+constexpr int kConfCols = 4096;          // columns per CTA (grid = ceil(V / kConfCols), <= kConfMaxCtas)
+
+struct ConfScratch {
+  float m[kConfMaxCtas], s[kConfMaxCtas];
+  unsigned int arrive;
+};
+
+__global__ void __launch_bounds__(kConfThreads)
+draft_confidence_kernel(const float* __restrict__ logits, const float* __restrict__ probs, int V,
+                        DevState* __restrict__ st, const GenParams* __restrict__ gpp, ConfScratch* __restrict__ cs,
+                        int j, int d_max, float* __restrict__ hidden, int hidden_ld,
+                        cudaGraphConditionalHandle next, int has_next) {
+  __shared__ float s_m[kConfThreads / 32], s_s[kConfThreads / 32];
+  __shared__ int s_last;
+  pdl_launch_dependents();
+  pdl_wait();
+  if (j == 0) {
+    const int n4 = (d_max - 1) * (hidden_ld >> 2);
+    float4* dst = reinterpret_cast<float4*>(hidden + 2 * (size_t)hidden_ld);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x)
+      dst[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  float conf;
+  if (logits != nullptr) {
+    const int per = (V + gridDim.x - 1) / gridDim.x;
+    const int lo = blockIdx.x * per, hi = min(V, lo + per);
+    float m = -INFINITY, s = 0.f;
+    for (int c = lo + threadIdx.x; c < hi; c += kConfThreads) {
+      const float v = logits[c];
+      if (v == -INFINITY) continue;
+      if (v > m) { s = s * expf(m - v) + 1.f; m = v; }
+      else s += expf(v - m);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float om = __shfl_xor_sync(0xffffffffu, m, o), os = __shfl_xor_sync(0xffffffffu, s, o);
+      lse_merge(m, s, om, os);
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) { s_m[warp] = m; s_s[warp] = s; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int w = 1; w < kConfThreads / 32; ++w) lse_merge(m, s, s_m[w], s_s[w]);
+      cs->m[blockIdx.x] = m;
+      cs->s[blockIdx.x] = s;
+      __threadfence();
+      s_last = atomicAdd(&cs->arrive, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last || threadIdx.x != 0) return;
+    __threadfence();
+    m = __ldcg(&cs->m[0]);
+    s = __ldcg(&cs->s[0]);
+    for (int b = 1; b < gridDim.x; ++b) lse_merge(m, s, __ldcg(&cs->m[b]), __ldcg(&cs->s[b]));
+    cs->arrive = 0;
+    conf = 1.0f / s;
+  } else {
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    conf = probs[st->tok[1 + j]];
+  }
+  if (j > 0 && st->d_stop <= j) return;   // eager launches only: an earlier draft already ended the round
+  const GenParams gp = *gpp;
+  st->conf[j] = conf;
+  const bool stop = j + 1 == d_max || is_eos(gp, st->tok[1 + j]) || conf < st->min_conf;
+  st->d_stop = stop ? j + 1 : d_max;
+  if (has_next) cudaGraphSetConditional(next, stop ? 0u : 1u);
 }
 
 }  // namespace lsk

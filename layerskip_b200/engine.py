@@ -26,6 +26,7 @@ class RoundOutput:
     draft: List[int]
     verified: List[int]
     kv_len: int
+    draft_confidence: Optional[List[float]] = None   # round_adaptive: confidence of each kept draft
 
 
 class Engine:
@@ -181,6 +182,23 @@ class Engine:
             emitted=list(out.emitted_ids[:out.n_emitted]),
             draft=list(out.draft_ids[:out.n_drafted]),
             verified=list(out.verified_ids[:out.n_drafted + 1]), kv_len=out.kv_len)
+
+    def round_adaptive(self, d_max: int, min_confidence: float) -> RoundOutput:
+        """A round that drafts up to `d_max` tokens and stops after the first draft that is an EOS or
+        whose probability under the distribution it was chosen from is below `min_confidence`
+        (Hugging Face's `assistant_confidence_threshold`); the draft steps after it do not run.  The
+        result is bit-identical to `round(n_drafted)` from the same state; `draft_confidence` holds
+        the kept drafts' confidences."""
+        out = _lib.lsk_round_out()
+        conf = (C.c_float * (_lib.LSK_MAX_SPEC + 1))()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_round_adaptive(self._h, int(d_max), float(min_confidence), C.byref(out), conf))
+        return RoundOutput(
+            n_drafted=out.n_drafted, n_matches=out.n_matches,
+            emitted=list(out.emitted_ids[:out.n_emitted]),
+            draft=list(out.draft_ids[:out.n_drafted]),
+            verified=list(out.verified_ids[:out.n_drafted + 1]), kv_len=out.kv_len,
+            draft_confidence=[float(x) for x in conf[:out.n_drafted]])
 
     KERNEL_CLASSES = ("qkv", "attention", "o_proj", "gate_up", "down", "lm_head", "small", "comm")
 

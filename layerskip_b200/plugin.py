@@ -47,6 +47,9 @@ class GenerationConfig:
     no_repeat_ngram_size: Optional[int] = None
     stop_words: Optional[List[str]] = None
     stop_token_ids: Optional[List[int]] = field(default=None)
+    # self-speculation only (not in the reference): stop a round's drafting after the first draft
+    # whose probability under the early-exit head is below this; 0 drafts num_speculations tokens
+    draft_confidence_threshold: float = 0.0
 
     def __post_init__(self):
         if self.stop_token_ids is None:

@@ -143,9 +143,11 @@ class B200SelfSpeculativeGenerationStrategy(GenerationStrategy):
         matches = drafted = 0
         self.last_rounds = []
         speculative_streamer = streamer is not None and hasattr(streamer, "delete")
+        # the reference's own GenerationConfig has no such field
+        threshold = float(getattr(cfg, "draft_confidence_threshold", 0.0) or 0.0)
         while len(output_ids) < cfg.max_steps:                       # :51
             d_req = min(cfg.num_speculations, cfg.max_steps - len(output_ids) - 1)   # :63-66
-            r = eng.round(d_req)
+            r = eng.round_adaptive(d_req, threshold) if threshold > 0 else eng.round(d_req)
             self.last_rounds.append(r)
             output_ids.extend(r.emitted)                             # :204-205
             matches += r.n_matches                                   # :80
