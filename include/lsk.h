@@ -280,7 +280,9 @@ int lsk_plan_gemm(int64_t n_rows, int64_t k, int32_t m, int32_t pro, int32_t epi
 /* Host-side launch plan of the attention kernel (pure host logic): split-KV factor (an engine
  * constant: results are batch-invariant only for a fixed partition), K/V ring depth, grid, shared
  * memory incl. the one-CTA-per-SM floor, 16-row blocks per CTA.  n_heads / n_kv_heads_local are the
- * tensor-parallel shard's head counts with the same GQA ratio as the model. */
+ * tensor-parallel shard's head counts with the same GQA ratio as the model.  ok = 0 when `m` rows
+ * do not fit, and for every `m` when the layout cannot run at all: a 16-token launch of its
+ * (head_dim, n_heads / n_kv_heads_local) does not fit shared memory (lsk_create refuses it). */
 typedef struct {
   int32_t ok, n_splits, ring_stages, grid, block, row_blocks, kv_refetched_per_row_block;
   int64_t smem_bytes, smem_limit;

@@ -440,6 +440,10 @@ static AttnLaunchPlan plan_attention_launch(int head_dim, int group, int M, int 
   if (kv_heads_local * n_splits <= sm_count && p.smem < (size_t)116 * 1024) p.smem = (size_t)116 * 1024;
   return p;
 }
+// Shared memory of the smallest launch a (head_dim, group) layout must run: the prompt pass launches
+// at least 16 tokens at a time (prompt_attn_rows) and a verify block carries up to kMaxRows = 16, both
+// at the 2-stage ring.  A layout above kSmemMax is refused by lsk_create.
+static size_t attn_layout_smem(int head_dim, int group) { return attn_smem_plan(head_dim, group, 16, 2).total; }
 
 // Attention over the paged cache: grid (kv heads, splits), the last split of a head to finish
 // merges; head_dim selects the instantiation, the shared-memory plan depends on (group, M).
@@ -1073,6 +1077,10 @@ int lsk_create(const lsk_config* cfg, lsk_engine** out) {
   if (c.tp_size < 1 || c.tp_rank < 0 || c.tp_rank >= c.tp_size) return fail(LSK_ERR_INVALID, "bad tp_rank/tp_size");
   if (c.n_heads % c.tp_size || c.n_kv_heads % c.tp_size || c.n_heads % c.n_kv_heads)
     return fail(LSK_ERR_INVALID, "heads (%d) / kv heads (%d) must divide by tp_size (%d)", c.n_heads, c.n_kv_heads, c.tp_size);
+  if (attn_layout_smem(c.head_dim, c.n_heads / c.n_kv_heads) > (size_t)kSmemMax)
+    return fail(LSK_ERR_INVALID, "attention: group %d (%d heads over %d kv heads) at head_dim %d needs %zu bytes of "
+                "shared memory for a 16-token launch, more than the %d available", c.n_heads / c.n_kv_heads,
+                c.n_heads, c.n_kv_heads, c.head_dim, attn_layout_smem(c.head_dim, c.n_heads / c.n_kv_heads), kSmemMax);
   if (c.inter % (c.tp_size * 8)) return fail(LSK_ERR_INVALID, "intermediate size %d must be a multiple of 8*tp_size", c.inter);
   if (c.hidden % 32 || c.hidden > 8192) return fail(LSK_ERR_INVALID, "hidden %d must be a multiple of 32 and <= 8192", c.hidden);
   if (c.vocab % c.tp_size) return fail(LSK_ERR_INVALID, "vocab must divide by tp_size");
@@ -2454,7 +2462,7 @@ int lsk_plan_attention(int32_t head_dim, int32_t n_heads, int32_t n_kv_heads_loc
   const int group = n_heads / n_kv_heads_local;
   const int splits = attn_default_splits(sm_count, n_kv_heads_local);
   const AttnLaunchPlan p = plan_attention_launch(head_dim, group, m, n_kv_heads_local, splits, kAttnMaxStages, sm_count);
-  out->ok = p.ok ? 1 : 0;
+  out->ok = (p.ok && attn_layout_smem(head_dim, group) <= (size_t)kSmemMax) ? 1 : 0;
   out->n_splits = splits;
   out->ring_stages = p.stages;
   out->grid = n_kv_heads_local * splits;

@@ -133,8 +133,14 @@ class RefModel:
     def attend(self, q: torch.Tensor, pos: torch.Tensor, K: torch.Tensor, V: torch.Tensor,
                n_keys: Optional[torch.Tensor] = None) -> torch.Tensor:
         """q [n, H, hd] at positions pos [n]; K / V [ctx, KV, hd] for positions 0 .. ctx-1.
-        Row i sees keys 0 .. pos[i] (or the first n_keys[i] keys) -> bf16 [n, H * hd]."""
+        Row i sees keys 0 .. pos[i] (or the first n_keys[i] keys) -> bf16 [n, H * hd].  Long
+        contexts run in row chunks that keep the float64 scores near 1 GiB (rows are independent)."""
         a = self.arch
+        step = max(1, 2 ** 27 // (a.heads * K.shape[0]))
+        if q.shape[0] > step:
+            return torch.cat([self.attend(q[i:i + step], pos[i:i + step], K, V,
+                                          None if n_keys is None else n_keys[i:i + step])
+                              for i in range(0, q.shape[0], step)])
         group = a.heads // a.kv_heads
         Kh = K.permute(1, 0, 2).repeat_interleave(group, 0)           # [H, ctx, hd]
         Vh = V.permute(1, 0, 2).repeat_interleave(group, 0)
