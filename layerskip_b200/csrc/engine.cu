@@ -154,15 +154,13 @@ struct lsk_engine {
   int* rank_idx = nullptr;
   int* d_zero = nullptr;
   int* d_prompt = nullptr;             // [max_ctx] prompt ids
-  float* score_lp = nullptr;           // lsk_score: [max_pos] log-probabilities (allocated on first use)
-  int* score_greedy = nullptr;         // lsk_score: [max_pos] arg-max ids
-  int* batch_buf = nullptr;            // lsk_score_batch: [8][max_pos] row ids, targets, row map, pieces of a group
-  unsigned int* piece_arrive = nullptr;  // lsk_score_batch: [128 pieces][kv heads] attention arrival counters
-  int* view_table = nullptr;           // lsk_score_prefixed: [max_pos] physical pages of a group's page-table views
-  // lsk_score_exits (allocated on first use, grown with the number of exits)
-  int exits_cap = 0;                   // exits the result arrays hold
-  float* exits_lp = nullptr;           // [exits_cap][max_pos] log-probabilities
-  int* exits_greedy = nullptr;         // [exits_cap][max_pos] arg-max ids
+  // scoring (allocated on first use; the result arrays grow with the number of exits)
+  int score_cap = 0;                   // exits the result arrays hold
+  float* score_lp = nullptr;           // [score_cap][max_pos] log-probabilities (packed scoring: row 0)
+  int* score_greedy = nullptr;         // [score_cap][max_pos] arg-max ids
+  int* batch_buf = nullptr;            // packed scoring: [8][max_pos] row ids, targets, row maps, pieces of a group
+  unsigned int* piece_arrive = nullptr;  // packed scoring: [128 pieces][kv heads] attention arrival counters
+  int* view_table = nullptr;           // packed scoring: [max_pos] physical pages of a group's page-table views
   int accept_cap = 0;                  // draft exits the acceptance buffers hold
   float* exits_accept = nullptr;       // [accept_cap][max_pos] acceptance probabilities
   float* exits_pd = nullptr;           // [accept_cap][128 or 16 rows][vocab] warped draft rows of the current chunk
@@ -615,16 +613,15 @@ static int launch_prompt_attention(lsk_engine* e, const __nv_bfloat16* q, int q_
   return LSK_OK;
 }
 
-// A chunk of rows from several sequences (lsk_score_batch), device pointers at the chunk's first row:
-// ids, per-row (position, first logical page), and the chunk's attention pieces (AttnPieces::pieces).
-// The first pages index page_table (nullptr: the engine's page table; lsk_score_prefixed passes
-// its table of page-table views).
+// A chunk of rows from several sequences (packed scoring), device pointers at the chunk's first row:
+// ids, per-row (position, first page), and the chunk's attention pieces (AttnPieces::pieces).  The
+// first pages index page_table, the group's table of page-table views.
 struct PackedChunk {
   const int* ids;
   const int2* row_map;
   const int4* pieces;
   int n_pieces, max_piece_rows;
-  const int* page_table = nullptr;
+  const int* page_table;
 };
 
 // Scoring at several exits in one pass (lsk_score_exits): at the top of layer layers[t] the first
@@ -646,7 +643,6 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool c
                                  const PackedChunk* pk = nullptr, const ChunkTaps* taps = nullptr) {
   const lsk_config& c = e->cfg;
   const bool tp = c.tp_size > 1;
-  const int* pk_pages = pk && pk->page_table ? pk->page_table : e->page_table;
   e->cur_class = CLS_MISC;
   CU(launch(e, embed_tokens_kernel, dim3(m), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
             pk ? pk->ids : (const int*)(e->d_prompt + c0), e->hidden_p, c.hidden));
@@ -686,7 +682,7 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool c
       a.q_rows = e->q_rows; a.kv_rows = e->kv_rows; a.n_kv_heads = e->kv_heads_l;
       if (pk) {
         a.row_map = pk->row_map;
-        a.page_table = pk_pages;
+        a.page_table = pk->page_table;
         TRY(launch_prefill_gemm<PF_EPI_QKV_MAP>(e, a));
       } else {
         TRY(launch_prefill_gemm<PF_EPI_QKV>(e, a));
@@ -700,7 +696,7 @@ static int enqueue_prefill_chunk(lsk_engine* e, int c0, int m, int n_run, bool c
       AttnArgs a{};
       a.q = e->q_p; a.q_ld = e->q_rows;
       a.out = reinterpret_cast<__nv_bfloat16*>(e->attn_c); a.out_canon = 1;
-      a.kpool = kp; a.vpool = vp; a.page_table = pk_pages; a.base_len = e->d_zero;
+      a.kpool = kp; a.vpool = vp; a.page_table = pk->page_table; a.base_len = e->d_zero;
       a.M = pk->max_piece_rows; a.group = e->group; a.n_kv_heads = e->kv_heads_l; a.n_splits = e->n_splits;
       a.scale = 1.0f / sqrtf((float)c.head_dim);
       const AttnPieces pz{pk->pieces, (e->group * kPfTokens + 15) / 16 * 16};
@@ -1052,6 +1048,66 @@ static int run_cached(lsk_engine* e, long long key, F enqueue) {
   return LSK_OK;
 }
 
+// Buffers allocated on first use: `bytes` at *p unless *p is already allocated.  On failure *p stays
+// null, so a later call tries again.
+template <typename T>
+static int alloc_once(T** p, size_t bytes) {
+  if (*p) return LSK_OK;
+  const cudaError_t er = cudaMalloc((void**)p, bytes);
+  if (er != cudaSuccess) {
+    *p = nullptr;
+    cudaGetLastError();
+    return fail(LSK_ERR_NOMEM, "cudaMalloc of %zu bytes failed: %s", bytes, cudaGetErrorString(er));
+  }
+  return LSK_OK;
+}
+// The same for a buffer that grows: the old allocation (if any) is freed first.
+template <typename T>
+static int realloc_grown(T** p, size_t bytes) {
+  if (*p) cudaFree(*p);
+  *p = nullptr;
+  return alloc_once(p, bytes);
+}
+// [16][vocab_l_pad] logits rows: the n-gram ban, sampling, adaptive drafts and the scoring heads
+static int ensure_logits(lsk_engine* e) { return alloc_once(&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4); }
+
+// Exit j's head on M residual rows at x: sequence rows r0 .., rows rc .. of the current chunk.
+using ExitHead = std::function<int(int j, const float* x, int r0, int rc, int M)>;
+
+// The prompt pass's route for rows 0 .. rows-1 of d_prompt (row i at position i) through layers
+// [0, E): prompts longer than one decode block go through the wgmma GEMMs 128 tokens per weight pass
+// (prefill_tc.cuh), short ones through the decode kernels in blocks of <= max_rows rows.  With k == 0
+// this is the prompt pass: no heads, and a chunk's last layer stops once its K/V rows are written.
+// With k > 0 the rows are scored at exits[0 .. k) (strictly increasing, exits[k - 1] == E), and
+// exit j's head runs where that exit's own pass would have stopped: wgmma chunks run to the end, with
+// a tap at the top of layer exits[j] for the earlier exits and the last head after the chunk, each on
+// the chunk's max_rows slices; decode blocks run it after layer exits[j] - 1.
+static int enqueue_prompt_rows(lsk_engine* e, int rows, int E, const int* exits, int k, const ExitHead& head) {
+  if (e->pf_tc && rows > e->max_rows) {
+    for (int c0 = 0; c0 < rows; c0 += kPfTokens) {
+      const int m = std::min(rows - c0, kPfTokens);
+      auto slices = [&](int j) -> int {
+        for (int r0 = 0; r0 < m; r0 += e->max_rows)
+          TRY(head(j, e->hidden_p + (size_t)r0 * e->cfg.hidden, c0 + r0, r0, std::min(m - r0, e->max_rows)));
+        return LSK_OK;
+      };
+      const ChunkTaps taps{exits, k - 1, slices};
+      TRY(enqueue_prefill_chunk(e, c0, m, E, k > 0, nullptr, k > 1 ? &taps : nullptr));
+      if (k > 0) TRY(slices(k - 1));
+    }
+  } else {
+    for (int c0 = 0; c0 < rows; c0 += e->max_rows) {
+      const int m = std::min(rows - c0, e->max_rows);
+      TRY(emit_embed(e, e->d_prompt + c0, e->hidden, m));
+      for (int l = 0, j = 0; l < E; ++l) {
+        TRY(enqueue_layer(e, l, 0, m, e->d_zero, c0));
+        if (j < k && exits[j] == l + 1) TRY(head(j++, e->hidden, c0, 0, m));
+      }
+    }
+  }
+  return LSK_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // C ABI
 // ---------------------------------------------------------------------------------------------
@@ -1315,8 +1371,8 @@ void lsk_destroy(lsk_engine* e) {
                   e->hidden, e->qbuf, e->attn_out, e->act, e->tp_buf, e->logits, e->logits_gath, e->logits_full, e->probs_d, e->probs_v, e->samp_scratch, e->cand_val,
                   e->cand_idx, e->gath_val, e->gath_idx, e->ban_val, e->ban_idx, e->rank_val, e->rank_idx,
                   e->d_zero, e->d_prompt, e->state, e->gen_dev, e->attn_part, e->attn_arrive,
-                  e->score_lp, e->score_greedy, e->batch_buf, e->piece_arrive, e->view_table, e->exits_lp, e->exits_greedy,
-                  e->exits_accept, e->exits_pd, e->exits_pv};
+                  e->score_lp, e->score_greedy, e->batch_buf, e->piece_arrive, e->view_table, e->exits_accept,
+                  e->exits_pd, e->exits_pv};
   for (void* p : ptrs) if (p) cudaFree(p);
   if (e->res_host) cudaFreeHost(e->res_host);
   if (e->ev0) cudaEventDestroy(e->ev0);
@@ -1548,25 +1604,16 @@ int lsk_begin(lsk_engine* e, const lsk_generation* gen) {
   if (gen->exit_layer > e->cfg.n_layers) return fail(LSK_ERR_INVALID, "exit_layer > n_layers");
   if (gen->no_repeat_ngram_size < 0 || gen->no_repeat_ngram_size > 16)
     return fail(LSK_ERR_INVALID, "no_repeat_ngram_size must be in [0, 16]");
-  if (gen->no_repeat_ngram_size > 0 && !e->logits) {
-    cudaError_t er = cudaMalloc((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4);
-    if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
-  }
+  if (gen->no_repeat_ngram_size > 0) TRY(ensure_logits(e));
   if (gen->sample) {
     if (!(gen->temperature > 0.f)) return fail(LSK_ERR_INVALID, "temperature must be > 0");
-    auto alloc0 = [&](float** p, size_t n) -> int {
-      if (*p) return LSK_OK;
-      cudaError_t er = cudaMalloc((void**)p, n * 4);
-      if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
-      return LSK_OK;
-    };
-    TRY(alloc0(&e->logits, (size_t)kMaxRows * e->vocab_l_pad));
-    TRY(alloc0(&e->probs_d, (size_t)kMaxRows * e->cfg.vocab));
-    TRY(alloc0(&e->probs_v, (size_t)kMaxRows * e->cfg.vocab));
-    TRY(alloc0(&e->samp_scratch, (size_t)e->cfg.vocab));
+    TRY(ensure_logits(e));
+    TRY(alloc_once(&e->probs_d, (size_t)kMaxRows * e->cfg.vocab * 4));
+    TRY(alloc_once(&e->probs_v, (size_t)kMaxRows * e->cfg.vocab * 4));
+    TRY(alloc_once(&e->samp_scratch, (size_t)e->cfg.vocab * 4));
     if (e->cfg.tp_size > 1) {
-      TRY(alloc0(&e->logits_gath, (size_t)e->cfg.tp_size * kMaxRows * e->vocab_l_pad));
-      TRY(alloc0(&e->logits_full, (size_t)kMaxRows * e->cfg.vocab));
+      TRY(alloc_once(&e->logits_gath, (size_t)e->cfg.tp_size * kMaxRows * e->vocab_l_pad * 4));
+      TRY(alloc_once(&e->logits_full, (size_t)kMaxRows * e->cfg.vocab * 4));
     }
   }
   e->gen = *gen;
@@ -1591,26 +1638,11 @@ int lsk_prefill(lsk_engine* e, const int32_t* ids, int32_t n) {
   if (n + 1 > e->cfg.max_ctx) return fail(LSK_ERR_CTX, "prompt of %d tokens exceeds max_ctx %d", n, e->cfg.max_ctx);
   for (int i = 0; i < n; ++i)
     if (ids[i] < 0 || ids[i] >= e->cfg.vocab) return fail(LSK_ERR_INVALID, "token id %d out of range", ids[i]);
-  const lsk_config& c = e->cfg;
   CU(cudaEventRecord(e->ev0, e->stream));
   CU(cudaMemcpyAsync(e->d_prompt, ids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
   // ids[0 .. n-2] through every layer; no LM head: the reference discards those logits too
-  // (self_speculation_generator.py:177).  Prompts longer than one decode block go through the
-  // wgmma GEMMs 128 tokens per weight pass (prefill_tc.cuh), short ones through the decode
-  // kernels in blocks of <= 16 rows.
-  if (e->pf_tc && n - 1 > e->max_rows) {
-    for (int c0 = 0; c0 < n - 1; c0 += kPfTokens) {
-      const int m = (n - 1 - c0) < kPfTokens ? (n - 1 - c0) : kPfTokens;
-      TRY(enqueue_prefill_chunk(e, c0, m, c.n_layers, false));
-    }
-  } else {
-    for (int c0 = 0; c0 < n - 1; c0 += e->max_rows) {
-      const int m = (n - 1 - c0) < e->max_rows ? (n - 1 - c0) : e->max_rows;
-      CU(launch(e, embed_tokens_kernel, dim3(m), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
-                (const int*)(e->d_prompt + c0), e->hidden, c.hidden));
-      for (int l = 0; l < c.n_layers; ++l) TRY(enqueue_layer(e, l, 0, m, e->d_zero, c0));
-    }
-  }
+  // (self_speculation_generator.py:177)
+  TRY(enqueue_prompt_rows(e, n - 1, e->cfg.n_layers, nullptr, 0, {}));
   set_state_kernel<<<1, 1, 0, e->stream>>>(e->state, n - 1, ids[n - 1], 0, n);
   CU(cudaGetLastError());
   CU(cudaEventRecord(e->ev1, e->stream));
@@ -1673,10 +1705,7 @@ int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_r
     CU(cudaMalloc((void**)&e->conf_scratch, sizeof(ConfScratch)));
     CU(cudaMemsetAsync(e->conf_scratch, 0, sizeof(ConfScratch), e->stream));
   }
-  if (!e->logits) {                       // greedy drafts materialise their logits row
-    cudaError_t er = cudaMalloc((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4);
-    if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
-  }
+  TRY(ensure_logits(e));                  // greedy drafts materialise their logits row
   // the threshold is read from device memory: one graph per round shape serves every threshold
   CU(cudaMemcpyAsync(&e->state->min_conf, &min_confidence, sizeof(float), cudaMemcpyHostToDevice, e->stream));
   const long long key = ((long long)E << 20) | ((long long)d_max << 8) | (e->gen.sample ? 4 : 0) | 8 | 1 |
@@ -1771,27 +1800,41 @@ int lsk_debug_forward_rows(lsk_engine* e, const int32_t* ids, int32_t m) {
   return LSK_OK;
 }
 
-// Scoring buffers, allocated on the first lsk_score / lsk_score_batch call.
-static int alloc_scoring(lsk_engine* e, bool batch) {
-  auto alloc0 = [&](void** p, size_t bytes) -> int {
-    if (*p) return LSK_OK;
-    cudaError_t er = cudaMalloc(p, bytes);
-    if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
-    return LSK_OK;
-  };
-  TRY(alloc0((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4));
-  TRY(alloc0((void**)&e->score_lp, (size_t)e->max_pos * 4));
-  TRY(alloc0((void**)&e->score_greedy, (size_t)e->max_pos * 4));
+// Scoring buffers, allocated on first use: the logits rows, result rows for k exits (regrown when a
+// call asks for more), and with `batch` packed scoring's group upload, arrival counters and view table.
+static int alloc_scoring(lsk_engine* e, int k, bool batch) {
+  const size_t P = (size_t)e->max_pos;
+  TRY(ensure_logits(e));
+  if (k > e->score_cap) {
+    e->score_cap = 0;
+    TRY(realloc_grown(&e->score_lp, (size_t)k * P * 4));
+    TRY(realloc_grown(&e->score_greedy, (size_t)k * P * 4));
+    e->score_cap = k;
+  }
   if (batch && !e->piece_arrive) {
-    TRY(alloc0((void**)&e->batch_buf, (size_t)8 * e->max_pos * 4));
-    TRY(alloc0((void**)&e->piece_arrive, (size_t)kPfTokens * e->kv_heads_l * 4));
+    TRY(alloc_once(&e->batch_buf, 8 * P * 4));
+    TRY(alloc_once(&e->view_table, P * 4));
+    TRY(alloc_once(&e->piece_arrive, (size_t)kPfTokens * e->kv_heads_l * 4));
     CU(cudaMemsetAsync(e->piece_arrive, 0, (size_t)kPfTokens * e->kv_heads_l * 4, e->stream));
   }
   return LSK_OK;
 }
 
+// lsk_score_exits' acceptance buffers for k - 1 draft exits: the acceptance rows and the warped draft
+// rows of a chunk, plus the warped full-depth rows of a slice.  A call with more exits regrows them.
+static int alloc_accept(lsk_engine* e, int k) {
+  if (k - 1 <= e->accept_cap) return LSK_OK;
+  const size_t V = (size_t)e->cfg.vocab, P = (size_t)e->max_pos, rows = e->pf_tc ? kPfTokens : kMaxRows;
+  e->accept_cap = 0;
+  TRY(realloc_grown(&e->exits_accept, (size_t)(k - 1) * P * 4));
+  TRY(realloc_grown(&e->exits_pd, (size_t)(k - 1) * rows * V * 4));
+  TRY(alloc_once(&e->exits_pv, (size_t)kMaxRows * V * 4));
+  e->accept_cap = k - 1;
+  return LSK_OK;
+}
+
 // LM head + log softmax on M residual rows at x: the log-probabilities of targets[0 .. M) and the
-// arg-max ids go to lp / greedy (score_lp / score_greedy unless given) from row r on.
+// arg-max ids go to lp / greedy (row 0 of score_lp / score_greedy unless given) from row r on.
 static int enqueue_score_head(lsk_engine* e, const float* x, int M, const int* targets, int r,
                               float* lp = nullptr, int* greedy = nullptr) {
   e->cur_class = CLS_LMHEAD;
@@ -1802,11 +1845,57 @@ static int enqueue_score_head(lsk_engine* e, const float* x, int M, const int* t
   return LSK_OK;
 }
 
-// Teacher-forced scoring (forward / forward_early of llama_model_utils.py:155-276 on the whole
-// sequence): rows 0 .. n-2 through layers [0, E), the final norm and the mma.sync LM head, then per
-// row the log-probability of the next id and the arg-max.  The rows take the prompt pass's route
-// (128-token wgmma chunks, or decode-kernel blocks of max_rows), so their K/V rows overwrite the
-// pool: any generation in progress ends here.
+// Teacher-forced scoring of one sequence (forward / forward_early of llama_model_utils.py:155-276 on
+// the whole sequence) at exits[0 .. k) in one pass: rows 0 .. n-2 take the prompt pass's route
+// through layers [0, exits[k - 1]), and at every exit the final norm, the mma.sync LM head, then per
+// row the log-probability of the next id and the arg-max.  Each exit's head runs where that exit's
+// own pass would have stopped (enqueue_prompt_rows), so every row is bit-identical to a one-exit call
+// at that exit.  With accept_out, each earlier exit's head also warps its logits into the chunk's
+// draft rows, and the full-depth head computes the acceptance probability of every draft row against
+// its own warped row.  The K/V rows overwrite the pool: any generation in progress ends here.
+static int score_sequence(lsk_engine* e, const int32_t* ids, int n, const int32_t* exits, int k,
+                          const lsk_generation* sampling, float* logprob_out, int32_t* greedy_out, float* accept_out) {
+  TRY(alloc_scoring(e, k, false));
+  if (accept_out) TRY(alloc_accept(e, k));
+  const int rows = n - 1, V = e->cfg.vocab;
+  const size_t P = (size_t)e->max_pos, pd_stride = (size_t)(e->pf_tc ? kPfTokens : kMaxRows) * V;
+  const WarpParams wp = accept_out ? WarpParams{sampling->temperature, sampling->top_k, sampling->top_p}
+                                   : WarpParams{1.f, 0, 1.f};
+  e->prefilled = false;
+  e->host_len = 0;
+  auto head = [&](int j, const float* x, int r0, int rc, int M) -> int {
+    TRY(enqueue_score_head(e, x, M, e->d_prompt + r0 + 1, r0, e->score_lp + j * P, e->score_greedy + j * P));
+    if (!accept_out || k == 1) return LSK_OK;
+    e->cur_class = CLS_MISC;
+    if (j + 1 < k) {
+      CU(launch(e, warp_rows_kernel, dim3(M), dim3(kSampleThreads), 0, (const float*)e->logits, e->vocab_l_pad, V,
+                wp, e->exits_pd + j * pd_stride + (size_t)rc * V));
+    } else {
+      CU(launch(e, accept_prob_kernel, dim3(M), dim3(kSampleThreads), 0, (const float*)e->logits, e->vocab_l_pad, V,
+                wp, (const float*)(e->exits_pd + (size_t)rc * V), pd_stride, k - 1, e->exits_pv,
+                e->exits_accept + r0, P));
+    }
+    return LSK_OK;
+  };
+  CU(cudaEventRecord(e->ev0, e->stream));
+  CU(cudaMemcpyAsync(e->d_prompt, ids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  TRY(enqueue_prompt_rows(e, rows, exits[k - 1], exits, k, head));
+  CU(cudaEventRecord(e->ev1, e->stream));
+  CU(cudaMemcpy2DAsync(logprob_out, (size_t)rows * 4, e->score_lp, P * 4, (size_t)rows * 4, k,
+                       cudaMemcpyDeviceToHost, e->stream));
+  if (greedy_out)
+    CU(cudaMemcpy2DAsync(greedy_out, (size_t)rows * 4, e->score_greedy, P * 4, (size_t)rows * 4, k,
+                         cudaMemcpyDeviceToHost, e->stream));
+  if (accept_out && k > 1)
+    CU(cudaMemcpy2DAsync(accept_out, (size_t)rows * 4, e->exits_accept, P * 4, (size_t)rows * 4, k - 1,
+                         cudaMemcpyDeviceToHost, e->stream));
+  CU(cudaStreamSynchronize(e->stream));
+  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
+  return LSK_OK;
+}
+
+// Teacher-forced scoring of one sequence at full depth or at an early exit: score_sequence with the
+// one exit E.
 int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer, float* logprob_out,
               int32_t* greedy_out) {
   if (!e || !ids || !logprob_out) return fail(LSK_ERR_INVALID, "null argument");
@@ -1818,39 +1907,8 @@ int lsk_score(lsk_engine* e, const int32_t* ids, int32_t n, int32_t exit_layer, 
   for (int i = 0; i < n; ++i)
     if (ids[i] < 0 || ids[i] >= c.vocab) return fail(LSK_ERR_INVALID, "token id %d out of range", ids[i]);
   if (!lsk_weights_complete(e)) return fail(LSK_ERR_STATE, "weights not fully loaded");
-  TRY(alloc_scoring(e, false));
-  const int E = exit_layer <= 0 ? c.n_layers : exit_layer;
-  const int rows = n - 1;
-  e->prefilled = false;
-  e->host_len = 0;
-  // M residual rows at x predict ids[r0 + 1 .. r0 + M]
-  auto head = [&](const float* x, int r0, int M) -> int {
-    return enqueue_score_head(e, x, M, e->d_prompt + r0 + 1, r0);
-  };
-  CU(cudaEventRecord(e->ev0, e->stream));
-  CU(cudaMemcpyAsync(e->d_prompt, ids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
-  if (e->pf_tc && rows > e->max_rows) {
-    for (int c0 = 0; c0 < rows; c0 += kPfTokens) {
-      const int m = std::min(rows - c0, kPfTokens);
-      TRY(enqueue_prefill_chunk(e, c0, m, E, true));
-      for (int r0 = 0; r0 < m; r0 += e->max_rows)
-        TRY(head(e->hidden_p + (size_t)r0 * c.hidden, c0 + r0, std::min(m - r0, e->max_rows)));
-    }
-  } else {
-    for (int c0 = 0; c0 < rows; c0 += e->max_rows) {
-      const int m = std::min(rows - c0, e->max_rows);
-      TRY(emit_embed(e, e->d_prompt + c0, e->hidden, m));
-      for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, 0, m, e->d_zero, c0));
-      TRY(head(e->hidden, c0, m));
-    }
-  }
-  CU(cudaEventRecord(e->ev1, e->stream));
-  CU(cudaMemcpyAsync(logprob_out, e->score_lp, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
-  if (greedy_out)
-    CU(cudaMemcpyAsync(greedy_out, e->score_greedy, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
-  CU(cudaStreamSynchronize(e->stream));
-  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
-  return LSK_OK;
+  const int32_t E = exit_layer <= 0 ? c.n_layers : exit_layer;
+  return score_sequence(e, ids, n, &E, 1, nullptr, logprob_out, greedy_out, nullptr);
 }
 
 // Attention pieces of nr packed rows at group rows r .. r + nr - 1, positions pos0 .., first page
@@ -1869,9 +1927,9 @@ static void add_pieces(std::vector<int4>& pieces, std::vector<int>& chunk_first,
 
 // The 128-row chunks of `rows` packed rows through layers [0, E): ids, row map and pieces on the
 // device at d_ids / d_map / d_pieces, the pieces' host copy in pieces / chunk_first (with its final
-// count), first pages indexing `pages` (nullptr: the engine's page table).  With targets every chunk
-// runs to the end and the score head runs on its max_rows slices (score_lp / score_greedy from row
-// c0 on); without, the chunks are a prompt pass that only writes K/V.
+// count), first pages indexing the view table `pages`.  With targets every chunk runs to the end and
+// the score head runs on its max_rows slices (score_lp / score_greedy from row c0 on); without, the
+// chunks are a prompt pass that only writes K/V.
 static int enqueue_packed_chunks(lsk_engine* e, int rows, int E, const int* d_ids, const int2* d_map,
                                  const int4* d_pieces, const std::vector<int4>& pieces,
                                  const std::vector<int>& chunk_first, const int* d_tgt, const int* pages) {
@@ -1889,15 +1947,172 @@ static int enqueue_packed_chunks(lsk_engine* e, int rows, int E, const int* d_id
   return LSK_OK;
 }
 
-// Teacher-forced scoring of many sequences on the wgmma prompt pass.  The rows of all sequences
-// (row i of a sequence predicts its id i + 1) are concatenated in input order and cut into 128-row
-// chunks.  A group is a run of sequences whose KV pages fit the pool together: sequence j owns the
-// logical pages [P_j, P_j + ceil((n_j - 1) / 64)), so its keys sit at positions 0 .. n_j - 2 of its
-// own page-table view, where lsk_score puts them, and a sequence's later chunks attend to the K/V
-// rows its earlier chunks wrote.  One upload per group carries the row ids, the targets, the row map
-// (position, first page) and the pieces of every chunk: maximal runs of one sequence's rows inside
-// a chunk, cut to the rows one prompt-attention launch holds.  Every row's arithmetic is that of
-// lsk_score on the same sequence's wgmma route.
+// Packed scoring's input: a prefix P and the branches B that continue it, pointers into the caller's
+// arrays; a branch's results go to the output arrays from row out_row on.
+struct ScoreBranch { const int32_t* ids; int n, out_row; };
+struct ScorePrefix { const int32_t* ids; int n; std::vector<ScoreBranch> br; };
+
+// Teacher-forced scoring of branches that continue prefixes, on the wgmma prompt pass through layers
+// [0, E).  Entry i of branch B on prefix P is the log-probability of B[i] after P + B[:i].  The
+// prefixes with their branches are taken in order in groups, as many as the KV pool and the view
+// table hold; a prefix whose branches do not all fit runs again in the next group.  With
+// s = len(P) - 1 and t = s mod 64, a group runs in two phases:
+//  * prefix phase: rows P[0 .. s) at positions 0 .. s - 1 write K/V only (the prompt pass: the last
+//    layer stops after its QKV GEMM, no head);
+//  * branch phase: rows [P[s]] + B[:-1] at positions s .. s + len(B) - 1 with targets B are scored.
+// The rows of a phase are concatenated in input order and cut into 128-row chunks; one upload per
+// group carries the row ids, the targets, the row maps (position, first page) and the pieces of every
+// chunk: maximal runs of one sequence's rows inside a chunk, cut to the rows one prompt-attention
+// launch holds.  Every sequence reads and writes keys through its own page-table view in view_table:
+// a prefix's view is its own pages; a branch's view is the prefix's s / 64 full pages, then (t > 0) a
+// page holding slots [0, t) of the prefix's partial page, then the branch's own pages.  The prefix's
+// first branch in the group adopts that partial page in place (its rows write slots >= t only); every
+// further branch gets a private copy of slots [0, t), made by one kv_copy_slots_kernel launch between
+// the phases.  A later chunk of a sequence attends to the K/V rows its earlier chunks wrote, at the
+// positions lsk_score puts them, so every row's arithmetic is that of lsk_score on P + B's wgmma route.
+static int score_packed(lsk_engine* e, int E, const std::vector<ScorePrefix>& pre, float* logprob_out,
+                        int32_t* greedy_out) {
+  TRY(alloc_scoring(e, 1, true));
+  const int m_attn = prompt_attn_rows(e->cfg.head_dim, e->group);
+  e->prefilled = false;
+  e->host_len = 0;
+
+  struct Member { const ScorePrefix* p; int b0, b1; };   // a prefix with its branches [b0, b1) in the group
+  std::vector<Member> grp;                 // the group being formed
+  std::vector<int32_t> up, view;           // the group's upload to batch_buf, its page-table views
+  std::vector<int4> pre_pieces, br_pieces, copies;
+  std::vector<int> pre_first, br_first, pre_view, br_view, br_row;
+  std::vector<float> lp_host;
+  std::vector<int32_t> gr_host;
+  // batch_buf sections start 16-byte aligned (row maps are int2, pieces and copies int4)
+  auto section = [&](size_t n) { const size_t o = up.size(); up.resize(o + (n + 3) / 4 * 4, 0); return o; };
+  auto run_group = [&](bool last) -> int {
+    view.clear(); copies.clear(); pre_pieces.clear(); br_pieces.clear();
+    pre_first.clear(); br_first.clear(); pre_view.clear(); br_view.clear(); br_row.clear();
+    int logical = 0, rp = 0, rb = 0;
+    auto new_page = [&]() { return e->page_table_host[logical++]; };
+    for (const Member& g : grp) {
+      const int s = g.p->n - 1, nf = s / kPageTokens, t = s % kPageTokens, pv = (int)view.size();
+      pre_view.push_back(pv);
+      for (int k = 0; k < (s + kPageTokens - 1) / kPageTokens; ++k) view.push_back(new_page());
+      rp += s;
+      for (int k = g.b0; k < g.b1; ++k) {
+        const int nb = g.p->br[k].n, bv = (int)view.size(), n_view = (s + nb + kPageTokens - 1) / kPageTokens;
+        for (int q = 0; q < nf; ++q) { const int page = view[pv + q]; view.push_back(page); }
+        if (t > 0) {
+          const int partial = view[pv + nf];
+          if (k == g.b0) {
+            view.push_back(partial);
+          } else {
+            const int page = new_page();
+            view.push_back(page);
+            copies.push_back(make_int4(partial, page, t, 0));
+          }
+        }
+        while ((int)view.size() - bv < n_view) view.push_back(new_page());
+        br_view.push_back(bv);
+        br_row.push_back(rb);
+        rb += nb;
+      }
+    }
+    up.clear();
+    const size_t o_pid = section(rp), o_pmap = section(2 * (size_t)rp);
+    const size_t o_bid = section(rb), o_btgt = section(rb), o_bmap = section(2 * (size_t)rb);
+    for (size_t gi = 0, r = 0, bi = 0; gi < grp.size(); ++gi) {
+      const Member& g = grp[gi];
+      const int32_t* P = g.p->ids;
+      const int s = g.p->n - 1;
+      for (int i = 0; i < s; ++i) {
+        up[o_pid + r + i] = P[i];
+        up[o_pmap + 2 * (r + i)] = i;
+        up[o_pmap + 2 * (r + i) + 1] = pre_view[gi];
+      }
+      add_pieces(pre_pieces, pre_first, (int)r, s, 0, pre_view[gi], m_attn);
+      r += s;
+      for (int k = g.b0; k < g.b1; ++k, ++bi) {
+        const int32_t* B = g.p->br[k].ids;
+        const int lb = g.p->br[k].n, r0 = br_row[bi];
+        for (int i = 0; i < lb; ++i) {
+          up[o_bid + r0 + i] = i ? B[i - 1] : P[s];
+          up[o_btgt + r0 + i] = B[i];
+          up[o_bmap + 2 * (r0 + i)] = s + i;
+          up[o_bmap + 2 * (r0 + i) + 1] = br_view[bi];
+        }
+        add_pieces(br_pieces, br_first, r0, lb, s, br_view[bi], m_attn);
+      }
+    }
+    pre_first.push_back((int)pre_pieces.size());
+    br_first.push_back((int)br_pieces.size());
+    const size_t o_ppc = section(4 * pre_pieces.size()), o_bpc = section(4 * br_pieces.size());
+    const size_t o_cp = section(4 * copies.size());
+    memcpy(up.data() + o_ppc, pre_pieces.data(), pre_pieces.size() * sizeof(int4));
+    memcpy(up.data() + o_bpc, br_pieces.data(), br_pieces.size() * sizeof(int4));
+    memcpy(up.data() + o_cp, copies.data(), copies.size() * sizeof(int4));
+    // every row owns a pool slot and needs at most 8 ints, so a group that fits the pool fits batch_buf
+    if (up.size() > (size_t)8 * e->max_pos)
+      return fail(LSK_ERR_INVALID, "packed scoring: group upload of %zu ints exceeds its buffer", up.size());
+    CU(cudaMemcpyAsync(e->batch_buf, up.data(), up.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    CU(cudaMemcpyAsync(e->view_table, view.data(), view.size() * 4, cudaMemcpyHostToDevice, e->stream));
+    const int* d = e->batch_buf;
+    auto i2 = [&](size_t o) { return reinterpret_cast<const int2*>(d + o); };
+    auto i4 = [&](size_t o) { return reinterpret_cast<const int4*>(d + o); };
+    TRY(enqueue_packed_chunks(e, rp, E, d + o_pid, i2(o_pmap), i4(o_ppc), pre_pieces, pre_first, nullptr,
+                              e->view_table));
+    if (!copies.empty()) {
+      e->cur_class = CLS_MISC;
+      CU(launch(e, kv_copy_slots_kernel, dim3((unsigned)copies.size(), E, 2 * e->kv_heads_l), dim3(128), 0, i4(o_cp),
+                e->kpool, e->vpool, e->pool_layer_elems, e->kv_heads_l, e->cfg.head_dim));
+    }
+    TRY(enqueue_packed_chunks(e, rb, E, d + o_bid, i2(o_bmap), i4(o_bpc), br_pieces, br_first, d + o_btgt,
+                              e->view_table));
+    if (last) CU(cudaEventRecord(e->ev1, e->stream));
+    lp_host.resize(rb);
+    gr_host.resize(rb);
+    CU(cudaMemcpyAsync(lp_host.data(), e->score_lp, (size_t)rb * 4, cudaMemcpyDeviceToHost, e->stream));
+    if (greedy_out)
+      CU(cudaMemcpyAsync(gr_host.data(), e->score_greedy, (size_t)rb * 4, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    for (size_t gi = 0, bi = 0; gi < grp.size(); ++gi)
+      for (int k = grp[gi].b0; k < grp[gi].b1; ++k, ++bi) {
+        const ScoreBranch& b = grp[gi].p->br[k];
+        memcpy(logprob_out + b.out_row, lp_host.data() + br_row[bi], (size_t)b.n * 4);
+        if (greedy_out) memcpy(greedy_out + b.out_row, gr_host.data() + br_row[bi], (size_t)b.n * 4);
+      }
+    grp.clear();
+    return LSK_OK;
+  };
+
+  CU(cudaEventRecord(e->ev0, e->stream));
+  int pages = 0, views = 0;   // pool pages and view entries the group uses
+  for (const ScorePrefix& p : pre) {
+    const int s = p.n - 1, nf = s / kPageTokens, t = s % kPageTokens, own = (s + kPageTokens - 1) / kPageTokens;
+    bool in_group = false;
+    for (int b = 0; b < (int)p.br.size(); ++b) {
+      const int n_view = (s + p.br[b].n + kPageTokens - 1) / kPageTokens;
+      // the prefix's pages come with its first branch in a group, which adopts the partial page
+      auto need_pages = [&]() { return in_group ? n_view - nf : own + n_view - nf - (t > 0 ? 1 : 0); };
+      auto need_views = [&]() { return in_group ? n_view : own + n_view; };
+      if (pages + need_pages() > e->n_pages || views + need_views() > e->max_pos) {
+        TRY(run_group(false));
+        pages = views = 0;
+        in_group = false;
+      }
+      pages += need_pages();
+      views += need_views();
+      if (!in_group) grp.push_back({&p, b, b});
+      in_group = true;
+      ++grp.back().b1;
+    }
+  }
+  TRY(run_group(true));
+  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
+  return LSK_OK;
+}
+
+// Teacher-forced scoring of many sequences on the wgmma prompt pass: sequence j is the branch
+// ids[1 ..] of the one-id prefix ids[0], so it has no prefix rows, its view is its own pages in
+// page-table order, and its rows are packed into shared 128-row chunks with the other sequences'
+// (score_packed).  Every row's arithmetic is that of lsk_score on the same sequence's wgmma route.
 int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs, int32_t exit_layer,
                     float* logprob_out, int32_t* greedy_out) {
   if (!e || !ids || !offsets || !logprob_out) return fail(LSK_ERR_INVALID, "null argument");
@@ -1918,73 +2133,15 @@ int lsk_score_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, i
       if (ids[i] < 0 || ids[i] >= c.vocab) return fail(LSK_ERR_INVALID, "sequence %d: token id %d out of range", j, ids[i]);
   }
   if (!lsk_weights_complete(e)) return fail(LSK_ERR_STATE, "weights not fully loaded");
-  TRY(alloc_scoring(e, true));
-  const int E = exit_layer <= 0 ? c.n_layers : exit_layer;
-  const int m_attn = prompt_attn_rows(c.head_dim, e->group);
-  e->prefilled = false;
-  e->host_len = 0;
-  std::vector<int32_t> up;        // the group's upload: ids [rows], targets [rows], row map [rows][2], pieces [][4]
-  std::vector<int4> pieces;
-  std::vector<int> chunk_first;   // first piece of each chunk, then the piece count
-  CU(cudaEventRecord(e->ev0, e->stream));
-  for (int j = 0, out_row = 0; j < n_seqs;) {
-    int k = j, pages = 0, rows = 0;
-    while (k < n_seqs) {
-      const int nr = offsets[k + 1] - offsets[k] - 1, np = (nr + kPageTokens - 1) / kPageTokens;
-      if (pages + np > e->n_pages) break;
-      pages += np; rows += nr; ++k;
-    }
-    up.assign((size_t)4 * rows, 0);
-    pieces.clear();
-    chunk_first.clear();
-    for (int s = j, r = 0, page = 0; s < k; ++s) {
-      const int32_t* sid = ids + offsets[s];
-      const int nr = offsets[s + 1] - offsets[s] - 1;
-      for (int i = 0; i < nr; ++i) {
-        up[r + i] = sid[i];
-        up[rows + r + i] = sid[i + 1];
-        up[2 * rows + 2 * (r + i)] = i;
-        up[2 * rows + 2 * (r + i) + 1] = page;
-      }
-      add_pieces(pieces, chunk_first, r, nr, 0, page, m_attn);
-      r += nr;
-      page += (nr + kPageTokens - 1) / kPageTokens;
-    }
-    chunk_first.push_back((int)pieces.size());
-    up.resize((size_t)4 * rows + 4 * pieces.size());
-    memcpy(up.data() + (size_t)4 * rows, pieces.data(), pieces.size() * sizeof(int4));
-    CU(cudaMemcpyAsync(e->batch_buf, up.data(), up.size() * 4, cudaMemcpyHostToDevice, e->stream));
-    const int* d_ids = e->batch_buf;
-    const int* d_tgt = e->batch_buf + rows;
-    const int2* d_map = reinterpret_cast<const int2*>(e->batch_buf + 2 * rows);
-    const int4* d_pieces = reinterpret_cast<const int4*>(e->batch_buf + 4 * rows);
-    TRY(enqueue_packed_chunks(e, rows, E, d_ids, d_map, d_pieces, pieces, chunk_first, d_tgt, nullptr));
-    if (k == n_seqs) CU(cudaEventRecord(e->ev1, e->stream));
-    CU(cudaMemcpyAsync(logprob_out + out_row, e->score_lp, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
-    if (greedy_out)
-      CU(cudaMemcpyAsync(greedy_out + out_row, e->score_greedy, (size_t)rows * 4, cudaMemcpyDeviceToHost, e->stream));
-    out_row += rows;
-    j = k;
-  }
-  CU(cudaStreamSynchronize(e->stream));
-  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
-  return LSK_OK;
+  // sequence j's n_j - 1 results start at row offsets[j] - j
+  std::vector<ScorePrefix> pre(n_seqs);
+  for (int j = 0; j < n_seqs; ++j)
+    pre[j] = {ids + offsets[j], 1, {{ids + offsets[j] + 1, offsets[j + 1] - offsets[j] - 1, offsets[j] - j}}};
+  return score_packed(e, exit_layer <= 0 ? c.n_layers : exit_layer, pre, logprob_out, greedy_out);
 }
 
-// Teacher-forced scoring of branches that continue shared prefixes, on the wgmma prompt pass.  With
-// s = len(P) - 1 and t = s mod 64, a group (prefixes with their branches, as many as the KV pool and
-// the view table hold) runs in two phases:
-//  * prefix phase: rows P[0 .. s) at positions 0 .. s - 1, packed into 128-row chunks, write K/V only
-//    (the prompt pass: the last layer stops after its QKV GEMM, no head);
-//  * branch phase: rows [P[s]] + B[:-1] at positions s .. s + len(B) - 1 with targets B, packed as in
-//    lsk_score_batch and scored.
-// Every sequence reads and writes keys through its own page-table view in view_table: a prefix's view
-// is its own pages; a branch's view is the prefix's s / 64 full pages, then (t > 0) a page holding
-// slots [0, t) of the prefix's partial page, then the branch's own pages.  The prefix's first branch
-// in the group adopts that partial page in place (its rows write slots >= t only); every further
-// branch gets a private copy of slots [0, t), made by one kv_copy_slots_kernel launch between the
-// phases.  Every row's arithmetic is that of lsk_score_batch on P + B, so the results are bit for bit
-// the same.  A prefix whose branches do not all fit runs again in the next group.
+// Teacher-forced scoring of branches that continue shared prefixes (score_packed): the results of
+// branch b start at row branch_offsets[b], and are bit for bit those of lsk_score_batch on P + B.
 int lsk_score_prefixed(lsk_engine* e, const int32_t* prefix_ids, const int32_t* prefix_offsets, int32_t n_prefixes,
                        const int32_t* branch_ids, const int32_t* branch_offsets, const int32_t* branch_prefix,
                        int32_t n_branches, int32_t exit_layer, float* logprob_out, int32_t* greedy_out) {
@@ -2013,7 +2170,8 @@ int lsk_score_prefixed(lsk_engine* e, const int32_t* prefix_ids, const int32_t* 
   TRY(check_parts("branch", branch_ids, branch_offsets, n_branches));
   auto plen = [&](int p) { return prefix_offsets[p + 1] - prefix_offsets[p]; };
   auto blen = [&](int b) { return branch_offsets[b + 1] - branch_offsets[b]; };
-  std::vector<std::vector<int>> kids(n_prefixes);   // each prefix's branches, in input order
+  std::vector<ScorePrefix> pre(n_prefixes);   // each prefix with its branches, in input order
+  for (int p = 0; p < n_prefixes; ++p) pre[p] = {prefix_ids + prefix_offsets[p], plen(p), {}};
   for (int b = 0; b < n_branches; ++b) {
     const int p = branch_prefix[b];
     if (p < 0 || p >= n_prefixes)
@@ -2021,195 +2179,15 @@ int lsk_score_prefixed(lsk_engine* e, const int32_t* prefix_ids, const int32_t* 
     if (plen(p) + blen(b) > c.max_ctx)
       return fail(LSK_ERR_CTX, "branch %d: prefix %d + branch = %d ids exceeds max_ctx %d", b, p, plen(p) + blen(b),
                   c.max_ctx);
-    kids[p].push_back(b);
+    pre[p].br.push_back({branch_ids + branch_offsets[b], blen(b), branch_offsets[b]});
   }
   for (int p = 0; p < n_prefixes; ++p)
-    if (kids[p].empty()) return fail(LSK_ERR_INVALID, "prefix %d has no branch", p);
+    if (pre[p].br.empty()) return fail(LSK_ERR_INVALID, "prefix %d has no branch", p);
   if (!lsk_weights_complete(e)) return fail(LSK_ERR_STATE, "weights not fully loaded");
-  TRY(alloc_scoring(e, true));
-  if (!e->view_table) {
-    const cudaError_t er = cudaMalloc((void**)&e->view_table, (size_t)e->max_pos * 4);
-    if (er != cudaSuccess) {
-      e->view_table = nullptr;
-      return fail(LSK_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(er));
-    }
-  }
-  const int E = exit_layer <= 0 ? c.n_layers : exit_layer;
-  const int m_attn = prompt_attn_rows(c.head_dim, e->group);
-  e->prefilled = false;
-  e->host_len = 0;
-
-  struct Member { int p; std::vector<int> br; };
-  std::vector<Member> grp;                 // the group being formed
-  std::vector<int32_t> up, view;           // the group's upload to batch_buf, its page-table views
-  std::vector<int4> pre_pieces, br_pieces, copies;
-  std::vector<int> pre_first, br_first, pre_view, br_view, br_row;
-  std::vector<float> lp_host;
-  std::vector<int32_t> gr_host;
-  // batch_buf sections start 16-byte aligned (row maps are int2, pieces and copies int4)
-  auto section = [&](size_t n) { const size_t o = up.size(); up.resize(o + (n + 3) / 4 * 4, 0); return o; };
-  auto run_group = [&](bool last) -> int {
-    view.clear(); copies.clear(); pre_pieces.clear(); br_pieces.clear();
-    pre_first.clear(); br_first.clear(); pre_view.clear(); br_view.clear(); br_row.clear();
-    int logical = 0, rp = 0, rb = 0;
-    auto new_page = [&]() { return e->page_table_host[logical++]; };
-    for (const Member& g : grp) {
-      const int s = plen(g.p) - 1, nf = s / kPageTokens, t = s % kPageTokens, pv = (int)view.size();
-      pre_view.push_back(pv);
-      for (int k = 0; k < (s + kPageTokens - 1) / kPageTokens; ++k) view.push_back(new_page());
-      rp += s;
-      for (size_t k = 0; k < g.br.size(); ++k) {
-        const int bv = (int)view.size(), n_view = (s + blen(g.br[k]) + kPageTokens - 1) / kPageTokens;
-        for (int q = 0; q < nf; ++q) { const int page = view[pv + q]; view.push_back(page); }
-        if (t > 0) {
-          const int partial = view[pv + nf];
-          if (k == 0) {
-            view.push_back(partial);
-          } else {
-            const int page = new_page();
-            view.push_back(page);
-            copies.push_back(make_int4(partial, page, t, 0));
-          }
-        }
-        while ((int)view.size() - bv < n_view) view.push_back(new_page());
-        br_view.push_back(bv);
-        br_row.push_back(rb);
-        rb += blen(g.br[k]);
-      }
-    }
-    up.clear();
-    const size_t o_pid = section(rp), o_pmap = section(2 * (size_t)rp);
-    const size_t o_bid = section(rb), o_btgt = section(rb), o_bmap = section(2 * (size_t)rb);
-    for (size_t gi = 0, r = 0, bi = 0; gi < grp.size(); ++gi) {
-      const int32_t* P = prefix_ids + prefix_offsets[grp[gi].p];
-      const int s = plen(grp[gi].p) - 1;
-      for (int i = 0; i < s; ++i) {
-        up[o_pid + r + i] = P[i];
-        up[o_pmap + 2 * (r + i)] = i;
-        up[o_pmap + 2 * (r + i) + 1] = pre_view[gi];
-      }
-      add_pieces(pre_pieces, pre_first, (int)r, s, 0, pre_view[gi], m_attn);
-      r += s;
-      for (int b : grp[gi].br) {
-        const int32_t* B = branch_ids + branch_offsets[b];
-        const int lb = blen(b), r0 = br_row[bi];
-        for (int i = 0; i < lb; ++i) {
-          up[o_bid + r0 + i] = i ? B[i - 1] : P[s];
-          up[o_btgt + r0 + i] = B[i];
-          up[o_bmap + 2 * (r0 + i)] = s + i;
-          up[o_bmap + 2 * (r0 + i) + 1] = br_view[bi];
-        }
-        add_pieces(br_pieces, br_first, r0, lb, s, br_view[bi], m_attn);
-        ++bi;
-      }
-    }
-    pre_first.push_back((int)pre_pieces.size());
-    br_first.push_back((int)br_pieces.size());
-    const size_t o_ppc = section(4 * pre_pieces.size()), o_bpc = section(4 * br_pieces.size());
-    const size_t o_cp = section(4 * copies.size());
-    memcpy(up.data() + o_ppc, pre_pieces.data(), pre_pieces.size() * sizeof(int4));
-    memcpy(up.data() + o_bpc, br_pieces.data(), br_pieces.size() * sizeof(int4));
-    memcpy(up.data() + o_cp, copies.data(), copies.size() * sizeof(int4));
-    // every row owns a pool slot and needs at most 8 ints, so a group that fits the pool fits batch_buf
-    if (up.size() > (size_t)8 * e->max_pos)
-      return fail(LSK_ERR_INVALID, "lsk_score_prefixed: group upload of %zu ints exceeds its buffer", up.size());
-    CU(cudaMemcpyAsync(e->batch_buf, up.data(), up.size() * 4, cudaMemcpyHostToDevice, e->stream));
-    CU(cudaMemcpyAsync(e->view_table, view.data(), view.size() * 4, cudaMemcpyHostToDevice, e->stream));
-    const int* d = e->batch_buf;
-    auto i2 = [&](size_t o) { return reinterpret_cast<const int2*>(d + o); };
-    auto i4 = [&](size_t o) { return reinterpret_cast<const int4*>(d + o); };
-    TRY(enqueue_packed_chunks(e, rp, E, d + o_pid, i2(o_pmap), i4(o_ppc), pre_pieces, pre_first, nullptr,
-                              e->view_table));
-    if (!copies.empty()) {
-      e->cur_class = CLS_MISC;
-      CU(launch(e, kv_copy_slots_kernel, dim3((unsigned)copies.size(), E, 2 * e->kv_heads_l), dim3(128), 0, i4(o_cp),
-                e->kpool, e->vpool, e->pool_layer_elems, e->kv_heads_l, c.head_dim));
-    }
-    TRY(enqueue_packed_chunks(e, rb, E, d + o_bid, i2(o_bmap), i4(o_bpc), br_pieces, br_first, d + o_btgt,
-                              e->view_table));
-    if (last) CU(cudaEventRecord(e->ev1, e->stream));
-    lp_host.resize(rb);
-    gr_host.resize(rb);
-    CU(cudaMemcpyAsync(lp_host.data(), e->score_lp, (size_t)rb * 4, cudaMemcpyDeviceToHost, e->stream));
-    if (greedy_out)
-      CU(cudaMemcpyAsync(gr_host.data(), e->score_greedy, (size_t)rb * 4, cudaMemcpyDeviceToHost, e->stream));
-    CU(cudaStreamSynchronize(e->stream));
-    for (size_t gi = 0, bi = 0; gi < grp.size(); ++gi)
-      for (int b : grp[gi].br) {
-        memcpy(logprob_out + branch_offsets[b], lp_host.data() + br_row[bi], (size_t)blen(b) * 4);
-        if (greedy_out) memcpy(greedy_out + branch_offsets[b], gr_host.data() + br_row[bi], (size_t)blen(b) * 4);
-        ++bi;
-      }
-    grp.clear();
-    return LSK_OK;
-  };
-
-  CU(cudaEventRecord(e->ev0, e->stream));
-  int pages = 0, views = 0;   // pool pages and view entries the group uses
-  for (int p = 0; p < n_prefixes; ++p) {
-    const int s = plen(p) - 1, nf = s / kPageTokens, t = s % kPageTokens, own = (s + kPageTokens - 1) / kPageTokens;
-    bool in_group = false;
-    for (int b : kids[p]) {
-      const int n_view = (s + blen(b) + kPageTokens - 1) / kPageTokens;
-      // the prefix's pages come with its first branch in a group, which adopts the partial page
-      auto need_pages = [&]() { return in_group ? n_view - nf : own + n_view - nf - (t > 0 ? 1 : 0); };
-      auto need_views = [&]() { return in_group ? n_view : own + n_view; };
-      if (pages + need_pages() > e->n_pages || views + need_views() > e->max_pos) {
-        TRY(run_group(false));
-        pages = views = 0;
-        in_group = false;
-      }
-      pages += need_pages();
-      views += need_views();
-      if (!in_group) grp.push_back({p, {}});
-      in_group = true;
-      grp.back().br.push_back(b);
-    }
-  }
-  TRY(run_group(true));
-  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
-  return LSK_OK;
+  return score_packed(e, exit_layer <= 0 ? c.n_layers : exit_layer, pre, logprob_out, greedy_out);
 }
 
-// lsk_score_exits buffers: result rows for k exits, and with `accept` the acceptance rows and the
-// warped draft rows of k - 1 exits.  Allocated on first use; a call with more exits regrows them.
-static int alloc_score_exits(lsk_engine* e, int k, bool accept) {
-  auto realloc0 = [&](void** p, size_t bytes) -> int {
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    cudaError_t er = cudaMalloc(p, bytes);
-    if (er != cudaSuccess) {
-      *p = nullptr;
-      cudaGetLastError();
-      return fail(LSK_ERR_NOMEM, "lsk_score_exits: cudaMalloc of %zu bytes failed: %s", bytes, cudaGetErrorString(er));
-    }
-    return LSK_OK;
-  };
-  const size_t V = (size_t)e->cfg.vocab, P = (size_t)e->max_pos;
-  if (!e->logits) TRY(realloc0((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4));
-  if (k > e->exits_cap) {
-    e->exits_cap = 0;
-    TRY(realloc0((void**)&e->exits_lp, (size_t)k * P * 4));
-    TRY(realloc0((void**)&e->exits_greedy, (size_t)k * P * 4));
-    e->exits_cap = k;
-  }
-  if (accept && k - 1 > e->accept_cap) {
-    const size_t rows = e->pf_tc ? kPfTokens : kMaxRows;
-    e->accept_cap = 0;
-    TRY(realloc0((void**)&e->exits_accept, (size_t)(k - 1) * P * 4));
-    TRY(realloc0((void**)&e->exits_pd, (size_t)(k - 1) * rows * V * 4));
-    if (!e->exits_pv) TRY(realloc0((void**)&e->exits_pv, (size_t)kMaxRows * V * 4));
-    e->accept_cap = k - 1;
-  }
-  return LSK_OK;
-}
-
-// Teacher-forced scoring at several exits in one pass: the rows take lsk_score's route for the
-// deepest exit, and the head of every earlier exit runs where that exit's own pass would have
-// stopped (wgmma chunks: a tap at the top of layer E_j; decode blocks: after layer E_j - 1), so
-// every row is bit-identical to lsk_score at that exit.  With accept_out, each earlier exit's
-// head also warps its logits into the chunk's draft rows, and the full-depth head computes the
-// acceptance probability of every draft row against its own warped row.
+// Teacher-forced scoring at several exits in one pass (score_sequence).
 int lsk_score_exits(lsk_engine* e, const int32_t* ids, int32_t n, const int32_t* exits, int32_t n_exits,
                     const lsk_generation* sampling, float* logprob_out, int32_t* greedy_out, float* accept_out) {
   if (!e || !ids || !exits || !logprob_out) return fail(LSK_ERR_INVALID, "null argument");
@@ -2240,65 +2218,7 @@ int lsk_score_exits(lsk_engine* e, const int32_t* ids, int32_t n, const int32_t*
                   exits[n_exits - 1]);
   }
   if (!lsk_weights_complete(e)) return fail(LSK_ERR_STATE, "weights not fully loaded");
-  TRY(alloc_score_exits(e, n_exits, accept_out != nullptr));
-  const int k = n_exits, E = exits[k - 1], rows = n - 1, V = c.vocab;
-  const bool tc = e->pf_tc && rows > e->max_rows;
-  const size_t P = (size_t)e->max_pos, pd_stride = (size_t)(tc ? kPfTokens : kMaxRows) * V;
-  const WarpParams wp = accept_out ? WarpParams{sampling->temperature, sampling->top_k, sampling->top_p}
-                                   : WarpParams{1.f, 0, 1.f};
-  e->prefilled = false;
-  e->host_len = 0;
-  // exit j's head on M residual rows at x: sequence rows r0 .., rows rc .. of the current chunk
-  auto head = [&](int j, const float* x, int r0, int rc, int M) -> int {
-    TRY(enqueue_score_head(e, x, M, e->d_prompt + r0 + 1, r0, e->exits_lp + j * P, e->exits_greedy + j * P));
-    if (!accept_out || k == 1) return LSK_OK;
-    e->cur_class = CLS_MISC;
-    if (j + 1 < k) {
-      CU(launch(e, warp_rows_kernel, dim3(M), dim3(kSampleThreads), 0, (const float*)e->logits, e->vocab_l_pad, V,
-                wp, e->exits_pd + j * pd_stride + (size_t)rc * V));
-    } else {
-      CU(launch(e, accept_prob_kernel, dim3(M), dim3(kSampleThreads), 0, (const float*)e->logits, e->vocab_l_pad, V,
-                wp, (const float*)(e->exits_pd + (size_t)rc * V), pd_stride, k - 1, e->exits_pv,
-                e->exits_accept + r0, P));
-    }
-    return LSK_OK;
-  };
-  CU(cudaEventRecord(e->ev0, e->stream));
-  CU(cudaMemcpyAsync(e->d_prompt, ids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
-  if (tc) {
-    for (int c0 = 0; c0 < rows; c0 += kPfTokens) {
-      const int m = std::min(rows - c0, kPfTokens);
-      auto slices = [&](int j) -> int {
-        for (int r0 = 0; r0 < m; r0 += e->max_rows)
-          TRY(head(j, e->hidden_p + (size_t)r0 * c.hidden, c0 + r0, r0, std::min(m - r0, e->max_rows)));
-        return LSK_OK;
-      };
-      const ChunkTaps taps{exits, k - 1, slices};
-      TRY(enqueue_prefill_chunk(e, c0, m, E, true, nullptr, k > 1 ? &taps : nullptr));
-      TRY(slices(k - 1));
-    }
-  } else {
-    for (int c0 = 0; c0 < rows; c0 += e->max_rows) {
-      const int m = std::min(rows - c0, e->max_rows);
-      TRY(emit_embed(e, e->d_prompt + c0, e->hidden, m));
-      for (int l = 0, j = 0; l < E; ++l) {
-        TRY(enqueue_layer(e, l, 0, m, e->d_zero, c0));
-        if (exits[j] == l + 1) TRY(head(j++, e->hidden, c0, 0, m));
-      }
-    }
-  }
-  CU(cudaEventRecord(e->ev1, e->stream));
-  CU(cudaMemcpy2DAsync(logprob_out, (size_t)rows * 4, e->exits_lp, P * 4, (size_t)rows * 4, k,
-                       cudaMemcpyDeviceToHost, e->stream));
-  if (greedy_out)
-    CU(cudaMemcpy2DAsync(greedy_out, (size_t)rows * 4, e->exits_greedy, P * 4, (size_t)rows * 4, k,
-                         cudaMemcpyDeviceToHost, e->stream));
-  if (accept_out && k > 1)
-    CU(cudaMemcpy2DAsync(accept_out, (size_t)rows * 4, e->exits_accept, P * 4, (size_t)rows * 4, k - 1,
-                         cudaMemcpyDeviceToHost, e->stream));
-  CU(cudaStreamSynchronize(e->stream));
-  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
-  return LSK_OK;
+  return score_sequence(e, ids, n, exits, n_exits, sampling, logprob_out, greedy_out, accept_out);
 }
 
 int lsk_kv_len(const lsk_engine* e, int32_t* len_out) {

@@ -20,23 +20,22 @@ SM_COUNT = 132                      # H100 SXM: one arg-max candidate slot per S
 def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling: bool = False,
                 keep_logits: bool = False, lm_head_tc: bool = False, prefill_tc: bool = True,
                 scoring: bool = False, batch_scoring: bool = False, score_exits: int = 0,
-                score_exits_sampled: bool = False, prefix_scoring: bool = False) -> Dict[str, int]:
+                score_exits_sampled: bool = False) -> Dict[str, int]:
     """Bytes the engine allocates on ONE rank.  Keys: weights, embed, lm_head, kv_pool, scratch,
     total (+ weights_source_peak: the largest single tensor staged on the GPU while loading).
     `scoring` adds what the first `lsk_score` call allocates: the logits rows (unless already
-    there) and one float + one int per position.  `batch_scoring` adds what the first
-    `lsk_score_batch` call allocates: the scoring buffers, eight ints per position (row ids,
-    targets, row map, attention pieces of a group) and one arrival counter per (piece, kv head)
-    of a 128-row chunk (nothing without the prompt pass, which refuses the call).  `score_exits`
-    = k adds what the first `lsk_score_exits` call with k exits allocates: the logits rows (unless
-    already there) and k floats + k ints per position; `score_exits_sampled` adds, for the k - 1
-    draft exits, one float per position and the warped draft rows of a chunk (128 rows with the
-    prompt pass, 16 without), plus 16 warped full-depth rows.  `prefix_scoring` adds what the first
-    `lsk_score_prefixed` call allocates: what `batch_scoring` adds, and one int per position for the
-    table of page-table views."""
+    there) and one float + one int per position.  `score_exits` = k adds what the first
+    `lsk_score_exits` call with k exits allocates: the logits rows and k floats + k ints per
+    position; the two share these result arrays, which grow to the most exits asked for.
+    `score_exits_sampled` adds, for the k - 1 draft exits, one float per position and the warped
+    draft rows of a chunk (128 rows with the prompt pass, 16 without), plus 16 warped full-depth
+    rows.  `batch_scoring` adds what the first `lsk_score_batch` or `lsk_score_prefixed` call
+    allocates: the scoring buffers, eight ints per position (row ids, targets, row maps, attention
+    pieces of a group), one int per position for the table of page-table views and one arrival
+    counter per (piece, kv head) of a 128-row chunk (nothing without the prompt pass, which
+    refuses the call)."""
     h, L = arch.hidden, arch.layers
-    prefix_scoring = prefix_scoring and prefill_tc and h % 64 == 0
-    batch_scoring = (batch_scoring or prefix_scoring) and prefill_tc and h % 64 == 0
+    batch_scoring = batch_scoring and prefill_tc and h % 64 == 0
     scoring = scoring or batch_scoring
     q_l = arch.heads // tp_size * arch.head_dim
     kv_l = arch.kv_heads // tp_size * arch.head_dim
@@ -74,17 +73,13 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
         scratch += 6 * 128 * h * 4 + 128 * q_l * 2 + 16384 * (h // 64 + (q_l + 63) // 64 + (inter_l + 63) // 64)
     if keep_logits or sampling or scoring or score_exits > 0:
         scratch += MAX_ROWS * vocab_l_pad * 4
-    if score_exits > 0:
-        scratch += 2 * score_exits * max_pos * 4            # per-exit log-probabilities + arg-max ids
-        if score_exits_sampled:
-            draft_rows = 128 if (prefill_tc and h % 64 == 0) else MAX_ROWS
-            scratch += (score_exits - 1) * (max_pos + draft_rows * arch.vocab) * 4 + MAX_ROWS * arch.vocab * 4
-    if scoring:
-        scratch += 2 * max_pos * 4                          # per-position log-probabilities + arg-max ids
+    result_exits = max(score_exits, 1 if scoring else 0)
+    scratch += 2 * result_exits * max_pos * 4               # per-exit log-probabilities + arg-max ids
+    if score_exits > 0 and score_exits_sampled:
+        draft_rows = 128 if (prefill_tc and h % 64 == 0) else MAX_ROWS
+        scratch += (score_exits - 1) * (max_pos + draft_rows * arch.vocab) * 4 + MAX_ROWS * arch.vocab * 4
     if batch_scoring:
-        scratch += 8 * max_pos * 4 + 128 * kvh_l * 4        # packed group arrays + piece arrival counters
-    if prefix_scoring:
-        scratch += max_pos * 4                              # page-table views of a group
+        scratch += 9 * max_pos * 4 + 128 * kvh_l * 4        # group arrays, view table, piece arrival counters
     if sampling:
         scratch += (2 * MAX_ROWS + 1) * arch.vocab * 4
         if tp_size > 1:

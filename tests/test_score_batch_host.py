@@ -96,7 +96,9 @@ def test_loglikelihood_batch_falls_back_without_the_prompt_pass(prefill_tc, hidd
 
 
 @pytest.mark.parametrize("name", ["llama2-7b", "llama3-8b", "tiny-gqa"])
-def test_plan_memory_batch_scoring_adds_exactly_the_batch_buffers(name):
+def test_plan_memory_batch_scoring_adds_exactly_the_packed_scoring_buffers(name):
+    """The buffers the first lsk_score_batch or lsk_score_prefixed call allocates: the group upload,
+    the view table and the piece arrival counters, on top of lsk_score's."""
     arch = ARCHS[name]
     max_ctx = 2048
     kvh = arch.kv_heads
@@ -105,7 +107,7 @@ def test_plan_memory_batch_scoring_adds_exactly_the_batch_buffers(name):
         base = plan_memory(arch, max_ctx=max_ctx, keep_logits=keep)
         assert plan_memory(arch, max_ctx=max_ctx, keep_logits=keep, batch_scoring=False) == base
         sc = plan_memory(arch, max_ctx=max_ctx, keep_logits=keep, scoring=True)
-        batch_only = 8 * max_ctx * 4 + 128 * kvh * 4
+        batch_only = 9 * max_ctx * 4 + 128 * kvh * 4          # group arrays, view table, arrival counters
         for scoring in (False, True):
             b = plan_memory(arch, max_ctx=max_ctx, keep_logits=keep, scoring=scoring, batch_scoring=True)
             assert b["scratch"] - sc["scratch"] == batch_only

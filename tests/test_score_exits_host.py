@@ -108,6 +108,9 @@ def test_plan_memory_score_exits_adds_exactly_its_buffers(name):
                 plain = plan_memory(arch, max_ctx=2048, keep_logits=keep, prefill_tc=prefill_tc, score_exits=k)
                 extra = 2 * k * 2048 * 4 + (0 if keep else 16 * vpad * 4)
                 assert plain["scratch"] - base["scratch"] == extra
+                # lsk_score's result arrays are row 0 of these: scoring as well costs nothing more
+                assert plan_memory(arch, max_ctx=2048, keep_logits=keep, prefill_tc=prefill_tc, score_exits=k,
+                                   scoring=True) == plain
                 assert plain["total"] - base["total"] == extra
                 assert {x: v for x, v in plain.items() if x not in ("scratch", "total")} == \
                     {x: v for x, v in base.items() if x not in ("scratch", "total")}

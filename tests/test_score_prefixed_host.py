@@ -1,13 +1,12 @@
 """CPU: the host side of prefix-shared scoring — how `Engine.loglikelihood_batch` groups requests by
 their cut context, what it passes to `score_prefixed`, how it maps results back, when it routes to
-`score_prefixed` rather than `score_batch`, validation before scoring, and the memory plan of the
-view table."""
+`score_prefixed` rather than `score_batch`, and validation before scoring.  (The memory plan of
+its buffers is `batch_scoring`'s, checked in test_score_batch_host.py.)"""
 import pytest
 import torch
 
 from layerskip_b200.engine import Engine
-from layerskip_b200.memory import plan_memory
-from layerskip_b200.weights import ARCHS, LlamaArch
+from layerskip_b200.weights import LlamaArch
 
 
 def _lp(ids):
@@ -138,20 +137,3 @@ def test_validation_comes_before_any_scoring():
             eng.loglikelihood_batch(bad)
     assert not eng.batch_calls and not eng.prefixed_calls and not eng.calls
 
-
-@pytest.mark.parametrize("name", ["llama2-7b", "llama3-8b", "tiny-gqa"])
-def test_plan_memory_prefix_scoring_adds_exactly_the_view_table(name):
-    arch = ARCHS[name]
-    max_ctx = 2048
-    for keep in (False, True):
-        base = plan_memory(arch, max_ctx=max_ctx, keep_logits=keep)
-        assert plan_memory(arch, max_ctx=max_ctx, keep_logits=keep, prefix_scoring=False) == base
-        for batch in (False, True):
-            b = plan_memory(arch, max_ctx=max_ctx, keep_logits=keep, batch_scoring=True)
-            p = plan_memory(arch, max_ctx=max_ctx, keep_logits=keep, batch_scoring=batch, prefix_scoring=True)
-            assert p["scratch"] - b["scratch"] == max_ctx * 4
-            assert p["total"] - b["total"] == max_ctx * 4
-            assert {k: v for k, v in p.items() if k not in ("scratch", "total")} == \
-                {k: v for k, v in base.items() if k not in ("scratch", "total")}
-    assert plan_memory(arch, max_ctx=max_ctx, prefill_tc=False, prefix_scoring=True) == \
-        plan_memory(arch, max_ctx=max_ctx, prefill_tc=False)
