@@ -290,6 +290,32 @@ typedef struct {
 int lsk_plan_attention(int32_t head_dim, int32_t n_heads, int32_t n_kv_heads_local, int32_t m,
                        int32_t sm_count, lsk_attn_plan* out);
 
+/* Device memory of one engine (one rank), in bytes per category: the packed layer weights (both
+ * layouts), the embedding and final norm, the LM head (both layouts), the paged KV pool, and
+ * everything else; total is their sum. */
+typedef struct {
+  int64_t weights, embed, lm_head, kv_pool, scratch, total;
+} lsk_memory_plan;
+/* What an engine is asked to do beyond what lsk_create allocates (a zeroed struct: nothing). */
+typedef struct {
+  int32_t lm_head_tc;        /* the opt-in wgmma LM head was asked for (LSK_LMHEAD_TC=1)          */
+  int32_t sampling;          /* lsk_begin with sample = 1                                         */
+  int32_t ngram_ban;         /* lsk_begin with no_repeat_ngram_size > 0                           */
+  int32_t adaptive;          /* lsk_round_adaptive                                                */
+  int32_t score_exits;       /* scoring with up to this many exits (lsk_score: 1), <= LSK_MAX_EXITS */
+  int32_t accept_exits;      /* lsk_score_exits with accept_out, up to this many exits            */
+  int32_t packed_scoring;    /* lsk_score_batch or lsk_score_prefixed                             */
+  int32_t tp_peer;           /* tp_size > 1: lsk_comm_init's peer region of the one-shot collectives */
+} lsk_memory_uses;
+/* Host-side plan of the device memory an engine with config `cfg` on a GPU with `sm_count` SMs
+ * allocates at lsk_create plus for `uses` (pure host logic; works without a GPU).  The flags it
+ * reads from cfg are the ones lsk_create reads; it refuses the configs lsk_create refuses, with the
+ * same codes and messages. */
+int lsk_plan_memory(const lsk_config* cfg, int32_t sm_count, const lsk_memory_uses* uses,
+                    lsk_memory_plan* out);
+/* The device memory the engine holds now, per category. */
+int lsk_memory_in_use(const lsk_engine* e, lsk_memory_plan* out);
+
 /* Stand-alone kernel entry points used by the micro-benchmarks and unit tests: run the skinny
  * GEMM (y[m, n] = x[m, k] . W[n, k]^T, fp32 out) on packed weights / the split-KV attention on
  * caller-provided device buffers. */

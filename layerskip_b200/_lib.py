@@ -81,6 +81,17 @@ class lsk_attn_plan(C.Structure):
                 ("smem_bytes", C.c_int64), ("smem_limit", C.c_int64)]
 
 
+class lsk_memory_plan(C.Structure):
+    _fields_ = [("weights", C.c_int64), ("embed", C.c_int64), ("lm_head", C.c_int64), ("kv_pool", C.c_int64),
+                ("scratch", C.c_int64), ("total", C.c_int64)]
+
+
+class lsk_memory_uses(C.Structure):
+    _fields_ = [("lm_head_tc", C.c_int32), ("sampling", C.c_int32), ("ngram_ban", C.c_int32),
+                ("adaptive", C.c_int32), ("score_exits", C.c_int32), ("accept_exits", C.c_int32),
+                ("packed_scoring", C.c_int32), ("tp_peer", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/lsk.h declares
 SIGNATURES = {
     "lsk_abi_version": (C.c_int, []),
@@ -123,6 +134,9 @@ SIGNATURES = {
                                 C.POINTER(lsk_gemm_plan)]),
     "lsk_plan_attention": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                      C.POINTER(lsk_attn_plan)]),
+    "lsk_plan_memory": (C.c_int, [C.POINTER(lsk_config), C.c_int32, C.POINTER(lsk_memory_uses),
+                                  C.POINTER(lsk_memory_plan)]),
+    "lsk_memory_in_use": (C.c_int, [C.c_void_p, C.POINTER(lsk_memory_plan)]),
     "lsk_test_pack": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
     "lsk_test_gemm": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int32,
                                 C.c_void_p, C.c_int32, C.POINTER(C.c_float)]),

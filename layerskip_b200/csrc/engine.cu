@@ -68,6 +68,63 @@ static int fail(int code, const char* fmt, ...) {
   } while (0)
 
 // ---------------------------------------------------------------------------------------------
+// device memory
+// ---------------------------------------------------------------------------------------------
+// The categories of lsk_memory_plan, in its field order.
+enum MemCat { MEM_WEIGHTS = 0, MEM_EMBED, MEM_LM_HEAD, MEM_KV_POOL, MEM_SCRATCH, MEM_CATS };
+struct MemBuf {
+  size_t bytes;
+  MemCat cat;
+};
+
+// Owner of device allocations: every pointer it hands out is recorded with its size and category
+// until it is freed, and whatever it still holds is freed when it is destroyed.
+class DeviceMem {
+ public:
+  cudaStream_t stream = nullptr;       // zero fills are enqueued here
+  DeviceMem() = default;
+  DeviceMem(const DeviceMem&) = delete;
+  DeviceMem& operator=(const DeviceMem&) = delete;
+  ~DeviceMem() { release(); }
+
+  // b.bytes at *p, zero-filled on `stream` when `zero`.  On failure *p is null.
+  template <typename T>
+  int alloc(T** p, const MemBuf& b, bool zero = false) {
+    const cudaError_t er = cudaMalloc((void**)p, b.bytes);
+    if (er != cudaSuccess) {
+      *p = nullptr;
+      cudaGetLastError();
+      return fail(LSK_ERR_NOMEM, "cudaMalloc of %zu bytes failed: %s", b.bytes, cudaGetErrorString(er));
+    }
+    held_.push_back({(void*)*p, b});
+    if (zero) CU(cudaMemsetAsync(*p, 0, b.bytes, stream));
+    return LSK_OK;
+  }
+  void free(void* p) {
+    for (size_t i = 0; i < held_.size(); ++i)
+      if (held_[i].p == p) {
+        cudaFree(p);
+        held_.erase(held_.begin() + i);
+        return;
+      }
+  }
+  void release() {
+    for (const Held& h : held_) cudaFree(h.p);
+    held_.clear();
+  }
+  void bytes_held(int64_t* cat) const {
+    for (const Held& h : held_) cat[h.b.cat] += (int64_t)h.b.bytes;
+  }
+
+ private:
+  struct Held {
+    void* p;
+    MemBuf b;
+  };
+  std::vector<Held> held_;
+};
+
+// ---------------------------------------------------------------------------------------------
 // engine
 // ---------------------------------------------------------------------------------------------
 struct LayerWeights {
@@ -89,13 +146,54 @@ struct GemmPlan {
   int n_tiles = 0, nsb = 0, K = 0;
 };
 
-struct lsk_engine {
-  lsk_config cfg{};
-  int sm_count = 0;
+// What an engine derives from its config, the SM count and which of its two optional paths it
+// takes: host arithmetic only (engine_shape), so lsk_plan_memory needs no device.
+struct EngineShape {
   // local (tensor-parallel shard) dimensions
   int heads_l = 0, kv_heads_l = 0, q_rows = 0, kv_rows = 0, inter_l = 0, vocab_l = 0,
       vocab_l_pad = 0, vocab_off = 0, group = 0, inter_l_pad = 0;
   int n_pages = 0, max_pos = 0, n_splits = 0;
+  size_t pool_layer_elems = 0;
+  // opt-in wgmma LM head (lmhead_tc.cuh): a second, canonical-layout copy of the head weights
+  bool lm_tc = false;
+  int lm_tc_tiles = 0, lm_tc_grid = 0, lm_tc_stages = 0;
+  int lm_cand = 0;                     // candidates produced by the wgmma LM head (its grid)
+  // tensor-core prefill: 128-token passes (on unless LSK_FLAG_NO_PREFILL_TC / LSK_PREFILL_TC=0)
+  bool pf_tc = false;
+  int pf_stages = 0;
+  int kst_h = 0, kst_q = 0, kst_i = 0;          // 64-wide k stages of hidden / q_rows / inter_l
+  int pf_t_qkv = 0, pf_t_h = 0, pf_t_gu = 0;     // 128-row tiles of qkv / hidden / gate-up outputs
+};
+
+// Every device buffer an engine can hold, with its size and category (mem_table): create_into, the
+// buffers allocated on first use and lsk_plan_memory all read their sizes from here.
+struct AttnBufs {
+  MemBuf part, arrive;                 // attention split partials, per-kv-head arrival counters
+};
+struct MemTable {
+  // at create, per layer; the canonical copies (*_c) with the prompt pass
+  MemBuf wqkv, wo, wgu, wd, norm, wqkv_c, wo_c, wgu_c, wd_c;
+  // at create with the prompt pass: [128][hidden] fp32 rows (hidden_p, tp_buf_p), O / down partials,
+  // q rows and the canonical activations
+  MemBuf rows_p, part_p, q_p, xn_c, attn_c, act_c;
+  MemBuf embed, final_norm, lm_head, lm_head_tc;   // lm_head_tc with the wgmma LM head
+  MemBuf kv_pool;                                   // each of kpool, vpool
+  MemBuf page_table, rope, hidden, qbuf, act, tp_buf;   // qbuf: also attn_out
+  AttnBufs attn;
+  MemBuf cand, gath, row_best, d_zero, d_prompt, state, gen_dev;   // cand / gath / row_best: each of val, idx
+  // on first use
+  MemBuf logits;          // at create with LSK_FLAG_KEEP_LOGITS; sampling, the n-gram ban, adaptive rounds, scoring
+  MemBuf vocab_rows;      // [16][vocab] fp32: probs_d, probs_v, logits_full (TP), exits_pv
+  MemBuf samp_scratch, logits_gath, conf_scratch;
+  MemBuf score_rows;      // per exit, each of score_lp, score_greedy
+  MemBuf accept_rows, draft_rows;                   // per draft exit: exits_accept, exits_pd
+  MemBuf batch_buf, view_table, piece_arrive;       // packed scoring
+  MemBuf peer_region;                               // lsk_comm_init with the one-shot collectives
+};
+
+struct lsk_engine : EngineShape {
+  lsk_config cfg{};
+  int sm_count = 0;
   int max_rows = kMaxRows;             // token rows one step can carry (8 when 16 do not fit)
   bool use_pdl = true, use_graph = true, keep_logits = false;
   bool pdl_break = false;              // launch the next kernel without the PDL attribute (graph conditional boundary)
@@ -105,16 +203,8 @@ struct lsk_engine {
   __nv_bfloat16* embed = nullptr;      // [vocab, hidden] natural (replicated)
   __nv_bfloat16* final_norm = nullptr;
   __nv_bfloat16* lm_head = nullptr;    // packed [vocab_l_pad, hidden]
-  // opt-in wgmma LM head (lmhead_tc.cuh): a second, canonical-layout copy of the head weights
-  bool lm_tc = false;
-  unsigned char* lm_head_tc = nullptr;   // [lm_tc_tiles][hidden / 64][16 KiB]
-  int lm_tc_tiles = 0, lm_tc_grid = 0, lm_tc_stages = 0;
+  unsigned char* lm_head_tc = nullptr;   // wgmma LM head: [lm_tc_tiles][hidden / 64][16 KiB]
   unsigned globals_loaded = 0;
-  // tensor-core prefill: 128-token passes (on unless LSK_FLAG_NO_PREFILL_TC / LSK_PREFILL_TC=0)
-  bool pf_tc = false;
-  int pf_stages = 0;
-  int kst_h = 0, kst_q = 0, kst_i = 0;          // 64-wide k stages of hidden / q_rows / inter_l
-  int pf_t_qkv = 0, pf_t_h = 0, pf_t_gu = 0;     // 128-row tiles of qkv / hidden / gate-up outputs
   float* hidden_p = nullptr;             // [128][hidden] fp32 residual rows of a prompt chunk
   float* tp_buf_p = nullptr;             // [128][hidden] fp32 row-parallel partial sums (TP)
   float* part_p = nullptr;               // [4 k-splits][128][hidden] fp32 partial tiles of the O / down GEMMs
@@ -125,7 +215,6 @@ struct lsk_engine {
 
   __nv_bfloat16* kpool = nullptr;      // [layer][page][kv_head][64][128]
   __nv_bfloat16* vpool = nullptr;
-  size_t pool_layer_elems = 0;
   int* page_table = nullptr;
   std::vector<int> page_table_host;    // host copy of page_table (prefix-shared scoring builds its views from it)
   float2* rope = nullptr;
@@ -171,7 +260,6 @@ struct lsk_engine {
   RoundResult* res_dev = nullptr;      // device alias of res_host
 
   GemmPlan p_qkv, p_o, p_gu, p_d, p_lm;
-  int lm_cand = 0;                     // candidates produced by the wgmma LM head (its grid)
   const float* cur_cand_val = nullptr;  // candidates of the last enqueued LM head (epilogue's, or the banned rows' arg-max)
   const int* cur_cand_idx = nullptr;
   int cur_n_cand = 0;
@@ -202,6 +290,29 @@ struct lsk_engine {
   bool profiling = false;
   int cur_class = 0;
   std::vector<std::pair<int, std::pair<cudaEvent_t, cudaEvent_t>>> prof_events;
+
+  MemTable sizes;                      // set by create_into
+  DeviceMem mem;                       // every device buffer above
+
+  lsk_engine() = default;
+  lsk_engine(const lsk_engine&) = delete;
+  lsk_engine& operator=(const lsk_engine&) = delete;
+  // lsk_destroy; also releases the temporary engines of the stand-alone test entry points on every
+  // return path.  Fields that were never set are skipped.
+  ~lsk_engine() {
+    if (stream) cudaStreamSynchronize(stream);
+    for (auto& kv : graphs) cudaGraphExecDestroy(kv.second);
+    for (void* p : peer_opened) if (p) cudaIpcCloseMemHandle(p);
+    if (comm) ncclCommDestroy(comm);
+    mem.release();
+    if (peer_err_host) cudaFreeHost(peer_err_host);
+    if (res_host) cudaFreeHost(res_host);
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+    if (stream) cudaStreamDestroy(stream);
+    if (body_stream) cudaStreamDestroy(body_stream);
+    cudaGetLastError();   // a half-built engine may have left a sticky-free error behind
+  }
 };
 
 enum { CLS_QKV = 0, CLS_ATTN = 1, CLS_O = 2, CLS_GATEUP = 3, CLS_DOWN = 4, CLS_LMHEAD = 5, CLS_MISC = 6, CLS_COMM = 7, CLS_COUNT = 8 };
@@ -482,13 +593,16 @@ static int launch_attention(lsk_engine* e, AttnArgs& a, int head_dim, const Attn
 }
 
 // Split partials + arrival counters of the attention kernel, sized for `rows` query tokens per
-// launch (the prompt pass's 128) at the engine's split count; the counters start at zero.
-static int alloc_attn_partials(lsk_engine* e, int kv_heads, int group, int head_dim, int rows) {
-  e->attn_part_cap = attn_part_floats(kv_heads, e->n_splits, (group * rows + 15) / 16 * 16, head_dim);
-  CU(cudaMalloc((void**)&e->attn_part, e->attn_part_cap * 4));
-  CU(cudaMalloc((void**)&e->attn_arrive, (size_t)kv_heads * 4));
-  CU(cudaMemsetAsync(e->attn_arrive, 0, (size_t)kv_heads * 4, e->stream));
-  return LSK_OK;
+// launch (the engine's: the prompt pass's 128) at `n_splits`.
+static AttnBufs attn_bufs(int kv_heads, int group, int head_dim, int n_splits, int rows) {
+  return {{attn_part_floats(kv_heads, n_splits, (group * rows + 15) / 16 * 16, head_dim) * 4, MEM_SCRATCH},
+          {(size_t)kv_heads * 4, MEM_SCRATCH}};
+}
+// The counters start at zero.
+static int alloc_attn_partials(lsk_engine* e, const AttnBufs& b) {
+  TRY(e->mem.alloc(&e->attn_part, b.part));
+  e->attn_part_cap = b.part.bytes / 4;
+  return e->mem.alloc(&e->attn_arrive, b.arrive, true);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1048,28 +1162,178 @@ static int run_cached(lsk_engine* e, long long key, F enqueue) {
   return LSK_OK;
 }
 
-// Buffers allocated on first use: `bytes` at *p unless *p is already allocated.  On failure *p stays
-// null, so a later call tries again.
-template <typename T>
-static int alloc_once(T** p, size_t bytes) {
-  if (*p) return LSK_OK;
-  const cudaError_t er = cudaMalloc((void**)p, bytes);
-  if (er != cudaSuccess) {
-    *p = nullptr;
-    cudaGetLastError();
-    return fail(LSK_ERR_NOMEM, "cudaMalloc of %zu bytes failed: %s", bytes, cudaGetErrorString(er));
+// ---------------------------------------------------------------------------------------------
+// shape, buffer sizes and memory plan (host only)
+// ---------------------------------------------------------------------------------------------
+// want_pf_tc / want_lm_tc: the prompt pass and the wgmma LM head are asked for; each is taken when
+// the hidden size fits it.
+static EngineShape engine_shape(const lsk_config& c, int sm_count, bool want_pf_tc, bool want_lm_tc) {
+  EngineShape s;
+  s.heads_l = c.n_heads / c.tp_size;
+  s.kv_heads_l = c.n_kv_heads / c.tp_size;
+  s.group = c.n_heads / c.n_kv_heads;
+  s.q_rows = s.heads_l * c.head_dim;
+  s.kv_rows = s.kv_heads_l * c.head_dim;
+  s.inter_l = c.inter / c.tp_size;
+  s.inter_l_pad = (s.inter_l + 31) / 32 * 32;   // K of the down projection (zero columns beyond inter_l)
+  s.vocab_l = c.vocab / c.tp_size;
+  s.vocab_l_pad = (s.vocab_l + 15) / 16 * 16;
+  s.vocab_off = c.tp_rank * s.vocab_l;
+  s.n_pages = (c.max_ctx + kPageTokens - 1) / kPageTokens;
+  s.max_pos = s.n_pages * kPageTokens;
+  // split-KV factor: a constant of the engine (results are batch-invariant only for a fixed
+  // partition).  The kernel is bound by per-SM load bandwidth and barrier latency, so the grid is
+  // ONE CTA per SM on as many SMs as possible — splits = floor(SMs / kv heads), at most 4 (7B: 32
+  // heads x 4 splits; an 8-way split's merge costs more than extra SMs bring).
+  s.n_splits = c.attn_splits > 0 ? c.attn_splits : attn_default_splits(sm_count, s.kv_heads_l);
+  if (s.n_splits > 8) s.n_splits = 8;
+  if (s.n_splits < 1) s.n_splits = 1;
+  s.pool_layer_elems = (size_t)s.n_pages * s.kv_heads_l * kPageTokens * c.head_dim;
+  if (want_lm_tc) {
+    // wgmma LM head: needs hidden % 64 == 0 and the 16-token B operand + a >= 3-stage ring in
+    // shared memory (hidden <= 5120)
+    int st = kTcMaxStages;
+    while (st >= 3 && lmhead_tc_smem_bytes(c.hidden, st) > (size_t)kSmemMax) --st;
+    if (c.hidden % kTcStageK == 0 && st >= 3) {
+      s.lm_tc = true;
+      s.lm_tc_stages = st;
+      s.lm_tc_tiles = (s.vocab_l + kTcTileRows - 1) / kTcTileRows;
+      const int waves = (s.lm_tc_tiles + sm_count - 1) / sm_count;
+      s.lm_tc_grid = (s.lm_tc_tiles + waves - 1) / waves;        // even waves
+      s.lm_cand = s.lm_tc_grid;
+    }
   }
-  return LSK_OK;
+  s.pf_tc = want_pf_tc && c.hidden % 64 == 0;
+  s.pf_stages = kPfMaxStages;
+  s.kst_h = c.hidden / 64;
+  s.kst_q = (s.q_rows + 63) / 64;
+  s.kst_i = (s.inter_l + 63) / 64;
+  s.pf_t_qkv = (s.q_rows + 2 * s.kv_rows + 127) / 128;
+  s.pf_t_h = (c.hidden + 127) / 128;
+  s.pf_t_gu = (2 * s.inter_l + 127) / 128;
+  return s;
+}
+
+static MemTable mem_table(const lsk_config& c, const EngineShape& s, int sm_count) {
+  const size_t h = c.hidden, V = c.vocab, P = s.max_pos, R = kMaxRows;
+  const MemCat W = MEM_WEIGHTS, S = MEM_SCRATCH;
+  MemTable t;
+  t.wqkv = {(size_t)(s.q_rows + 2 * s.kv_rows) * h * 2, W};
+  t.wo = {h * s.q_rows * 2, W};
+  t.wgu = {(size_t)2 * s.inter_l * h * 2, W};
+  t.wd = {h * s.inter_l_pad * 2, W};
+  t.norm = {h * 2, W};
+  t.wqkv_c = {(size_t)s.pf_t_qkv * s.kst_h * kCanonStageBytes, W};
+  t.wo_c = {(size_t)s.pf_t_h * s.kst_q * kCanonStageBytes, W};
+  t.wgu_c = {(size_t)s.pf_t_gu * s.kst_h * kCanonStageBytes, W};
+  t.wd_c = {(size_t)s.pf_t_h * s.kst_i * kCanonStageBytes, W};
+  t.rows_p = {(size_t)kPfTokens * h * 4, S};
+  t.part_p = {(size_t)4 * kPfTokens * h * 4, S};
+  t.q_p = {(size_t)kPfTokens * s.q_rows * 2, S};
+  t.xn_c = {(size_t)s.kst_h * kCanonStageBytes, S};
+  t.attn_c = {(size_t)s.kst_q * kCanonStageBytes, S};
+  t.act_c = {(size_t)s.kst_i * kCanonStageBytes, S};
+  t.embed = {V * h * 2, MEM_EMBED};
+  t.final_norm = {h * 2, MEM_EMBED};
+  t.lm_head = {(size_t)s.vocab_l_pad * h * 2, MEM_LM_HEAD};
+  t.lm_head_tc = {(size_t)s.lm_tc_tiles * kTcTileRows * h * 2, MEM_LM_HEAD};
+  t.kv_pool = {s.pool_layer_elems * c.n_layers * 2, MEM_KV_POOL};
+  t.page_table = {(size_t)s.n_pages * 4, S};
+  t.rope = {P * (c.head_dim / 2) * sizeof(float2), S};
+  t.hidden = {(R + 1) * h * 4, S};
+  t.qbuf = {R * s.q_rows * 2, S};
+  t.act = {R * s.inter_l_pad * 2, S};
+  t.tp_buf = {R * h * 4, S};
+  t.attn = attn_bufs(s.kv_heads_l, s.group, c.head_dim, s.n_splits, std::max(kMaxRows, kPfTokens));
+  t.cand = {(size_t)sm_count * R * 4, S};
+  t.gath = {(size_t)c.tp_size * R * 4, S};
+  t.row_best = {R * 4, S};
+  t.d_zero = {4, S};
+  t.d_prompt = {P * 4, S};
+  t.state = {sizeof(DevState), S};
+  t.gen_dev = {sizeof(GenParams), S};
+  t.logits = {R * s.vocab_l_pad * 4, S};
+  t.vocab_rows = {R * V * 4, S};
+  t.samp_scratch = {V * 4, S};
+  t.logits_gath = {(size_t)c.tp_size * R * s.vocab_l_pad * 4, S};
+  t.conf_scratch = {sizeof(ConfScratch), S};
+  t.score_rows = {P * 4, S};
+  t.accept_rows = {P * 4, S};
+  t.draft_rows = {(size_t)(s.pf_tc ? kPfTokens : kMaxRows) * V * 4, S};
+  t.batch_buf = {8 * P * 4, S};
+  t.view_table = {P * 4, S};
+  t.piece_arrive = {(size_t)kPfTokens * s.kv_heads_l * 4, S};
+  t.peer_region = {peer_region_layout(c.tp_size, c.hidden).total, S};
+  return t;
+}
+
+// Bytes per category (MemCat order) of what create_into allocates, plus what the uses allocate.
+static void plan_memory(const lsk_config& c, const EngineShape& s, const MemTable& t, const lsk_memory_uses& u,
+                        int64_t* cat) {
+  auto add = [&](const MemBuf& b, size_t n) { cat[b.cat] += (int64_t)(b.bytes * n); };
+  const size_t L = c.n_layers;
+  for (const MemBuf& b : {t.wqkv, t.wo, t.wgu, t.wd}) add(b, L);
+  add(t.norm, 2 * L);
+  if (s.pf_tc) {
+    for (const MemBuf& b : {t.wqkv_c, t.wo_c, t.wgu_c, t.wd_c}) add(b, L);
+    add(t.rows_p, 2);
+    for (const MemBuf& b : {t.part_p, t.q_p, t.xn_c, t.attn_c, t.act_c}) add(b, 1);
+  }
+  for (const MemBuf& b : {t.embed, t.final_norm, t.lm_head}) add(b, 1);
+  if (s.lm_tc) add(t.lm_head_tc, 1);
+  add(t.kv_pool, 2);
+  for (const MemBuf& b : {t.page_table, t.rope, t.hidden, t.act, t.tp_buf, t.attn.part, t.attn.arrive, t.d_zero,
+                          t.d_prompt, t.state, t.gen_dev})
+    add(b, 1);
+  add(t.qbuf, 2);
+  add(t.cand, 2);
+  add(t.gath, 2);
+  add(t.row_best, 4);
+  const bool packed = u.packed_scoring && s.pf_tc;     // without the prompt pass the call is refused
+  const int score_k = std::max({u.score_exits, u.accept_exits, packed ? 1 : 0});
+  const int draft_k = u.accept_exits - 1;
+  if ((c.flags & LSK_FLAG_KEEP_LOGITS) || u.sampling || u.ngram_ban || u.adaptive || score_k > 0) add(t.logits, 1);
+  if (u.sampling) {
+    add(t.vocab_rows, 2);
+    add(t.samp_scratch, 1);
+    if (c.tp_size > 1) {
+      add(t.logits_gath, 1);
+      add(t.vocab_rows, 1);
+    }
+  }
+  if (u.adaptive) add(t.conf_scratch, 1);
+  add(t.score_rows, 2 * (size_t)score_k);
+  if (draft_k > 0) {
+    add(t.accept_rows, draft_k);
+    add(t.draft_rows, draft_k);
+    add(t.vocab_rows, 1);
+  }
+  if (packed)
+    for (const MemBuf& b : {t.batch_buf, t.view_table, t.piece_arrive}) add(b, 1);
+  if (u.tp_peer && c.tp_size > 1) add(t.peer_region, 1);
+}
+
+static lsk_memory_plan plan_of(const int64_t* cat) {
+  return {cat[MEM_WEIGHTS], cat[MEM_EMBED], cat[MEM_LM_HEAD], cat[MEM_KV_POOL], cat[MEM_SCRATCH],
+          cat[MEM_WEIGHTS] + cat[MEM_EMBED] + cat[MEM_LM_HEAD] + cat[MEM_KV_POOL] + cat[MEM_SCRATCH]};
+}
+
+// Buffers allocated on first use: nothing to do once *p is allocated.  On failure *p stays null, so a
+// later call tries again.
+template <typename T>
+static int alloc_once(lsk_engine* e, T** p, const MemBuf& b, bool zero = false) {
+  return *p ? LSK_OK : e->mem.alloc(p, b, zero);
 }
 // The same for a buffer that grows: the old allocation (if any) is freed first.
 template <typename T>
-static int realloc_grown(T** p, size_t bytes) {
-  if (*p) cudaFree(*p);
+static int realloc_grown(lsk_engine* e, T** p, const MemBuf& b) {
+  e->mem.free(*p);
   *p = nullptr;
-  return alloc_once(p, bytes);
+  return e->mem.alloc(p, b);
 }
+static MemBuf times(MemBuf b, size_t n) { return {b.bytes * n, b.cat}; }
 // [16][vocab_l_pad] logits rows: the n-gram ban, sampling, adaptive drafts and the scoring heads
-static int ensure_logits(lsk_engine* e) { return alloc_once(&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4); }
+static int ensure_logits(lsk_engine* e) { return alloc_once(e, &e->logits, e->sizes.logits); }
 
 // Exit j's head on M residual rows at x: sequence rows r0 .., rows rc .. of the current chunk.
 using ExitHead = std::function<int(int j, const float* x, int r0, int rc, int M)>;
@@ -1118,9 +1382,8 @@ const char* lsk_last_error(void) { return g_last_error.c_str(); }
 
 static int create_into(lsk_engine* e, const lsk_config& c);
 
-int lsk_create(const lsk_config* cfg, lsk_engine** out) {
-  if (!cfg || !out) return fail(LSK_ERR_INVALID, "null argument");
-  const lsk_config& c = *cfg;
+// The configs lsk_create and lsk_plan_memory accept.
+static int check_config(const lsk_config& c) {
   if (c.head_dim != 128 && c.head_dim != 64 && c.head_dim != 32)
     return fail(LSK_ERR_INVALID, "head_dim %d unsupported (32, 64 or 128)", c.head_dim);
   if (c.rope_scaling < LSK_ROPE_DEFAULT || c.rope_scaling > LSK_ROPE_LLAMA3)
@@ -1141,10 +1404,15 @@ int lsk_create(const lsk_config* cfg, lsk_engine** out) {
   if (c.hidden % 32 || c.hidden > 8192) return fail(LSK_ERR_INVALID, "hidden %d must be a multiple of 32 and <= 8192", c.hidden);
   if (c.vocab % c.tp_size) return fail(LSK_ERR_INVALID, "vocab must divide by tp_size");
   if (c.n_layers < 1 || c.max_ctx < 2) return fail(LSK_ERR_INVALID, "bad n_layers / max_ctx");
+  return LSK_OK;
+}
 
+int lsk_create(const lsk_config* cfg, lsk_engine** out) {
+  if (!cfg || !out) return fail(LSK_ERR_INVALID, "null argument");
+  TRY(check_config(*cfg));
   // everything that can fail half-way runs in create_into(); a failure releases what was built
   lsk_engine* e = new lsk_engine();
-  const int st = create_into(e, c);
+  const int st = create_into(e, *cfg);
   if (st != LSK_OK) {
     const std::string why = g_last_error;
     lsk_destroy(e);
@@ -1152,6 +1420,28 @@ int lsk_create(const lsk_config* cfg, lsk_engine** out) {
     return st;
   }
   *out = e;
+  return LSK_OK;
+}
+
+int lsk_plan_memory(const lsk_config* cfg, int32_t sm_count, const lsk_memory_uses* uses, lsk_memory_plan* out) {
+  if (!cfg || !uses || !out) return fail(LSK_ERR_INVALID, "null argument");
+  TRY(check_config(*cfg));
+  if (sm_count < 1) return fail(LSK_ERR_INVALID, "sm_count %d must be >= 1", sm_count);
+  if (uses->score_exits < 0 || uses->score_exits > LSK_MAX_EXITS || uses->accept_exits < 0 ||
+      uses->accept_exits > LSK_MAX_EXITS)
+    return fail(LSK_ERR_INVALID, "score_exits and accept_exits must be in [0, %d]", LSK_MAX_EXITS);
+  const EngineShape s = engine_shape(*cfg, sm_count, !(cfg->flags & LSK_FLAG_NO_PREFILL_TC), uses->lm_head_tc != 0);
+  int64_t cat[MEM_CATS] = {};
+  plan_memory(*cfg, s, mem_table(*cfg, s, sm_count), *uses, cat);
+  *out = plan_of(cat);
+  return LSK_OK;
+}
+
+int lsk_memory_in_use(const lsk_engine* e, lsk_memory_plan* out) {
+  if (!e || !out) return fail(LSK_ERR_INVALID, "null argument");
+  int64_t cat[MEM_CATS] = {};
+  e->mem.bytes_held(cat);
+  *out = plan_of(cat);
   return LSK_OK;
 }
 
@@ -1187,130 +1477,89 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
     }
     if (e->ablate) fprintf(stderr, "[lsk] LSK_ABLATE=%s: kernel classes skipped, outputs are NOT valid\n", env);
   }
-  e->heads_l = c.n_heads / c.tp_size;
-  e->kv_heads_l = c.n_kv_heads / c.tp_size;
-  e->group = c.n_heads / c.n_kv_heads;
-  e->q_rows = e->heads_l * c.head_dim;
-  e->kv_rows = e->kv_heads_l * c.head_dim;
-  e->inter_l = c.inter / c.tp_size;
-  e->inter_l_pad = (e->inter_l + 31) / 32 * 32;   // K of the down projection (zero columns beyond inter_l)
-  e->vocab_l = c.vocab / c.tp_size;
-  e->vocab_l_pad = (e->vocab_l + 15) / 16 * 16;
-  e->vocab_off = c.tp_rank * e->vocab_l;
-  e->n_pages = (c.max_ctx + kPageTokens - 1) / kPageTokens;
-  e->max_pos = e->n_pages * kPageTokens;
-  // split-KV factor: a constant of the engine (results are batch-invariant only for a fixed
-  // partition).  The kernel is bound by per-SM load bandwidth and barrier latency, so the grid is
-  // ONE CTA per SM on as many SMs as possible — splits = floor(SMs / kv heads), at most 4 (7B: 32
-  // heads x 4 splits; an 8-way split's merge costs more than extra SMs bring).
-  e->n_splits = c.attn_splits > 0 ? c.attn_splits : attn_default_splits(e->sm_count, e->kv_heads_l);
-  if (e->n_splits > 8) e->n_splits = 8;
-  if (e->n_splits < 1) e->n_splits = 1;
+  const char* lm_env = getenv("LSK_LMHEAD_TC");
+  const char* pf_env = getenv("LSK_PREFILL_TC");
+  const bool want_lm_tc = lm_env && atoi(lm_env) != 0;
+  static_cast<EngineShape&>(*e) = engine_shape(c, e->sm_count, !(c.flags & LSK_FLAG_NO_PREFILL_TC) &&
+                                               !(pf_env && atoi(pf_env) == 0), want_lm_tc);
+  // without the wgmma LM head's fit, stay on the mma.sync kernel, loudly
+  if (want_lm_tc && !e->lm_tc)
+    fprintf(stderr, "[lsk] LSK_LMHEAD_TC ignored: hidden %d does not fit the wgmma LM head\n", c.hidden);
+  e->sizes = mem_table(c, *e, e->sm_count);
 
   e->p_qkv = make_plan(e->q_rows + 2 * e->kv_rows, c.hidden);
   e->p_o = make_plan(c.hidden, e->q_rows);
   e->p_gu = make_plan(2 * e->inter_l, c.hidden);
   e->p_d = make_plan(c.hidden, e->inter_l_pad);
   e->p_lm = make_plan(e->vocab_l_pad, c.hidden);
-  if (getenv("LSK_LMHEAD_TC") && atoi(getenv("LSK_LMHEAD_TC")) != 0) {
-    // wgmma LM head: needs hidden % 64 == 0 and the 16-token B operand + a >= 3-stage ring in
-    // shared memory (hidden <= 5120); otherwise stay on the mma.sync kernel, loudly
-    int st = kTcMaxStages;
-    while (st >= 3 && lmhead_tc_smem_bytes(c.hidden, st) > (size_t)kSmemMax) --st;
-    if (c.hidden % kTcStageK == 0 && st >= 3) {
-      e->lm_tc = true;
-      e->lm_tc_stages = st;
-      e->lm_tc_tiles = (e->vocab_l + kTcTileRows - 1) / kTcTileRows;
-      const int waves = (e->lm_tc_tiles + e->sm_count - 1) / e->sm_count;
-      e->lm_tc_grid = (e->lm_tc_tiles + waves - 1) / waves;        // even waves
-      e->lm_cand = e->lm_tc_grid;
-    } else {
-      fprintf(stderr, "[lsk] LSK_LMHEAD_TC ignored: hidden %d does not fit the wgmma LM head\n", c.hidden);
-    }
-  }
   e->max_rows = plan_sched(2, kMaxRows, PRO_RMS, EPI_QKV, e->p_qkv, e->sm_count).ok ? kMaxRows : 8;
-  {
-    const char* env = getenv("LSK_PREFILL_TC");
-    e->pf_tc = !(c.flags & LSK_FLAG_NO_PREFILL_TC) && !(env && atoi(env) == 0) && c.hidden % 64 == 0;
-    e->pf_stages = kPfMaxStages;
-    e->kst_h = c.hidden / 64;
-    e->kst_q = (e->q_rows + 63) / 64;
-    e->kst_i = (e->inter_l + 63) / 64;
-    e->pf_t_qkv = (e->q_rows + 2 * e->kv_rows + 127) / 128;
-    e->pf_t_h = (c.hidden + 127) / 128;
-    e->pf_t_gu = (2 * e->inter_l + 127) / 128;
-  }
 
   CU(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
   CU(cudaEventCreate(&e->ev0));
   CU(cudaEventCreate(&e->ev1));
 
-  auto alloc = [&](void** p, size_t bytes) -> int {
-    cudaError_t er = cudaMalloc(p, bytes);
-    if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(er));
-    cudaMemsetAsync(*p, 0, bytes, e->stream);
-    return LSK_OK;
-  };
-  const size_t h = c.hidden;
+  e->mem.stream = e->stream;
+
+  const MemTable& t = e->sizes;
+  auto alloc = [&](auto** p, const MemBuf& b) { return e->mem.alloc(p, b, true); };   // zero-filled
   e->layers.resize(c.n_layers);
   for (auto& L : e->layers) {
-    TRY(alloc((void**)&L.wqkv, (size_t)(e->q_rows + 2 * e->kv_rows) * h * 2));
-    TRY(alloc((void**)&L.wo, h * e->q_rows * 2));
-    TRY(alloc((void**)&L.wgu, (size_t)2 * e->inter_l * h * 2));
-    TRY(alloc((void**)&L.wd, h * e->inter_l_pad * 2));
-    TRY(alloc((void**)&L.ln1, h * 2));
-    TRY(alloc((void**)&L.ln2, h * 2));
+    TRY(alloc(&L.wqkv, t.wqkv));
+    TRY(alloc(&L.wo, t.wo));
+    TRY(alloc(&L.wgu, t.wgu));
+    TRY(alloc(&L.wd, t.wd));
+    TRY(alloc(&L.ln1, t.norm));
+    TRY(alloc(&L.ln2, t.norm));
     if (e->pf_tc) {
-      TRY(alloc((void**)&L.wqkv_c, (size_t)e->pf_t_qkv * e->kst_h * kCanonStageBytes));
-      TRY(alloc((void**)&L.wo_c, (size_t)e->pf_t_h * e->kst_q * kCanonStageBytes));
-      TRY(alloc((void**)&L.wgu_c, (size_t)e->pf_t_gu * e->kst_h * kCanonStageBytes));
-      TRY(alloc((void**)&L.wd_c, (size_t)e->pf_t_h * e->kst_i * kCanonStageBytes));
+      TRY(alloc(&L.wqkv_c, t.wqkv_c));
+      TRY(alloc(&L.wo_c, t.wo_c));
+      TRY(alloc(&L.wgu_c, t.wgu_c));
+      TRY(alloc(&L.wd_c, t.wd_c));
     }
   }
   if (e->pf_tc) {
-    TRY(alloc((void**)&e->hidden_p, (size_t)kPfTokens * h * 4));
-    TRY(alloc((void**)&e->tp_buf_p, (size_t)kPfTokens * h * 4));
-    TRY(alloc((void**)&e->part_p, (size_t)4 * kPfTokens * h * 4));
-    TRY(alloc((void**)&e->q_p, (size_t)kPfTokens * e->q_rows * 2));
-    TRY(alloc((void**)&e->xn_c, (size_t)e->kst_h * kCanonStageBytes));
-    TRY(alloc((void**)&e->attn_c, (size_t)e->kst_q * kCanonStageBytes));
-    TRY(alloc((void**)&e->act_c, (size_t)e->kst_i * kCanonStageBytes));
+    TRY(alloc(&e->hidden_p, t.rows_p));
+    TRY(alloc(&e->tp_buf_p, t.rows_p));
+    TRY(alloc(&e->part_p, t.part_p));
+    TRY(alloc(&e->q_p, t.q_p));
+    TRY(alloc(&e->xn_c, t.xn_c));
+    TRY(alloc(&e->attn_c, t.attn_c));
+    TRY(alloc(&e->act_c, t.act_c));
     CU(cudaFuncSetAttribute(prefill_gemm_tc_kernel<PF_EPI_QKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
     CU(cudaFuncSetAttribute(prefill_gemm_tc_kernel<PF_EPI_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
     CU(cudaFuncSetAttribute(prefill_gemm_tc_kernel<PF_EPI_SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
     CU(cudaFuncSetAttribute(prefill_gemm_tc_kernel<PF_EPI_QKV_MAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
   }
-  TRY(alloc((void**)&e->embed, (size_t)c.vocab * h * 2));
-  TRY(alloc((void**)&e->final_norm, h * 2));
-  TRY(alloc((void**)&e->lm_head, (size_t)e->vocab_l_pad * h * 2));
+  TRY(alloc(&e->embed, t.embed));
+  TRY(alloc(&e->final_norm, t.final_norm));
+  TRY(alloc(&e->lm_head, t.lm_head));
   if (e->lm_tc) {
-    TRY(alloc((void**)&e->lm_head_tc, (size_t)e->lm_tc_tiles * kTcTileRows * h * 2));
+    TRY(alloc(&e->lm_head_tc, t.lm_head_tc));
     CU(cudaFuncSetAttribute(lmhead_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
   }
-  e->pool_layer_elems = (size_t)e->n_pages * e->kv_heads_l * kPageTokens * c.head_dim;
-  TRY(alloc((void**)&e->kpool, e->pool_layer_elems * c.n_layers * 2));
-  TRY(alloc((void**)&e->vpool, e->pool_layer_elems * c.n_layers * 2));
-  TRY(alloc((void**)&e->page_table, (size_t)e->n_pages * 4));
-  TRY(alloc((void**)&e->rope, (size_t)e->max_pos * (c.head_dim / 2) * sizeof(float2)));
-  TRY(alloc((void**)&e->hidden, (size_t)(kMaxRows + 1) * h * 4));
-  TRY(alloc((void**)&e->qbuf, (size_t)kMaxRows * e->q_rows * 2));
-  TRY(alloc((void**)&e->attn_out, (size_t)kMaxRows * e->q_rows * 2));
-  TRY(alloc_attn_partials(e, e->kv_heads_l, e->group, c.head_dim, std::max(kMaxRows, 128)));
-  TRY(alloc((void**)&e->act, (size_t)kMaxRows * e->inter_l_pad * 2));   // pad columns stay zero
-  TRY(alloc((void**)&e->tp_buf, (size_t)kMaxRows * h * 4));
-  if (e->keep_logits) TRY(alloc((void**)&e->logits, (size_t)kMaxRows * e->vocab_l_pad * 4));
-  TRY(alloc((void**)&e->cand_val, (size_t)e->sm_count * kMaxRows * 4));
-  TRY(alloc((void**)&e->cand_idx, (size_t)e->sm_count * kMaxRows * 4));
-  TRY(alloc((void**)&e->gath_val, (size_t)c.tp_size * kMaxRows * 4));
-  TRY(alloc((void**)&e->gath_idx, (size_t)c.tp_size * kMaxRows * 4));
-  TRY(alloc((void**)&e->ban_val, kMaxRows * 4));
-  TRY(alloc((void**)&e->ban_idx, kMaxRows * 4));
-  TRY(alloc((void**)&e->rank_val, kMaxRows * 4));
-  TRY(alloc((void**)&e->rank_idx, kMaxRows * 4));
-  TRY(alloc((void**)&e->d_zero, 4));
-  TRY(alloc((void**)&e->d_prompt, (size_t)e->max_pos * 4));
-  TRY(alloc((void**)&e->state, sizeof(DevState)));
-  TRY(alloc((void**)&e->gen_dev, sizeof(GenParams)));
+  TRY(alloc(&e->kpool, t.kv_pool));
+  TRY(alloc(&e->vpool, t.kv_pool));
+  TRY(alloc(&e->page_table, t.page_table));
+  TRY(alloc(&e->rope, t.rope));
+  TRY(alloc(&e->hidden, t.hidden));
+  TRY(alloc(&e->qbuf, t.qbuf));
+  TRY(alloc(&e->attn_out, t.qbuf));
+  TRY(alloc_attn_partials(e, t.attn));
+  TRY(alloc(&e->act, t.act));   // pad columns stay zero
+  TRY(alloc(&e->tp_buf, t.tp_buf));
+  if (e->keep_logits) TRY(alloc(&e->logits, t.logits));
+  TRY(alloc(&e->cand_val, t.cand));
+  TRY(alloc(&e->cand_idx, t.cand));
+  TRY(alloc(&e->gath_val, t.gath));
+  TRY(alloc(&e->gath_idx, t.gath));
+  TRY(alloc(&e->ban_val, t.row_best));
+  TRY(alloc(&e->ban_idx, t.row_best));
+  TRY(alloc(&e->rank_val, t.row_best));
+  TRY(alloc(&e->rank_idx, t.row_best));
+  TRY(alloc(&e->d_zero, t.d_zero));
+  TRY(alloc(&e->d_prompt, t.d_prompt));
+  TRY(alloc(&e->state, t.state));
+  TRY(alloc(&e->gen_dev, t.gen_dev));
   CU(cudaHostAlloc((void**)&e->res_host, sizeof(RoundResult), cudaHostAllocMapped));
   memset(e->res_host, 0, sizeof(RoundResult));
   CU(cudaHostGetDevicePointer((void**)&e->res_dev, e->res_host, 0));
@@ -1351,38 +1600,7 @@ static int create_into(lsk_engine* e, const lsk_config& c) {
   return LSK_OK;
 }
 
-void lsk_destroy(lsk_engine* e) {
-  if (!e) return;
-  if (e->stream) cudaStreamSynchronize(e->stream);
-  for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
-  for (void* p : e->peer_opened) if (p) cudaIpcCloseMemHandle(p);
-  if (e->peer_region) cudaFree(e->peer_region);
-  if (e->peer_err_host) cudaFreeHost(e->peer_err_host);
-  if (e->comm) ncclCommDestroy(e->comm);
-  for (auto& L : e->layers) {
-    cudaFree(L.wqkv); cudaFree(L.wo); cudaFree(L.wgu); cudaFree(L.wd); cudaFree(L.ln1); cudaFree(L.ln2);
-    cudaFree(L.wqkv_c); cudaFree(L.wo_c); cudaFree(L.wgu_c); cudaFree(L.wd_c);
-  }
-  {
-    void* pf[] = {e->hidden_p, e->tp_buf_p, e->part_p, e->q_p, e->xn_c, e->attn_c, e->act_c};
-    for (void* p : pf) if (p) cudaFree(p);
-  }
-  void* ptrs[] = {e->embed, e->final_norm, e->lm_head, e->lm_head_tc, e->kpool, e->vpool, e->page_table, e->rope,
-                  e->hidden, e->qbuf, e->attn_out, e->act, e->tp_buf, e->logits, e->logits_gath, e->logits_full, e->probs_d, e->probs_v, e->samp_scratch, e->cand_val,
-                  e->cand_idx, e->gath_val, e->gath_idx, e->ban_val, e->ban_idx, e->rank_val, e->rank_idx,
-                  e->d_zero, e->d_prompt, e->state, e->gen_dev, e->attn_part, e->attn_arrive,
-                  e->score_lp, e->score_greedy, e->batch_buf, e->piece_arrive, e->view_table, e->exits_accept,
-                  e->exits_pd, e->exits_pv};
-  for (void* p : ptrs) if (p) cudaFree(p);
-  if (e->res_host) cudaFreeHost(e->res_host);
-  if (e->ev0) cudaEventDestroy(e->ev0);
-  if (e->ev1) cudaEventDestroy(e->ev1);
-  if (e->stream) cudaStreamDestroy(e->stream);
-  if (e->body_stream) cudaStreamDestroy(e->body_stream);
-  if (e->conf_scratch) cudaFree(e->conf_scratch);
-  cudaGetLastError();   // a half-built engine may have left a sticky-free error behind
-  delete e;
-}
+void lsk_destroy(lsk_engine* e) { delete e; }
 
 int lsk_comm_unique_id(uint8_t id_out[128]) {
   static_assert(sizeof(ncclUniqueId) == 128, "ncclUniqueId size");
@@ -1397,24 +1615,19 @@ int lsk_comm_unique_id(uint8_t id_out[128]) {
 static int peer_setup(lsk_engine* e) {
   const int tp = e->cfg.tp_size, rank = e->cfg.tp_rank;
   if (tp > kMaxPeers) return fail(LSK_ERR_INVALID, "one-shot collectives support at most %d ranks", kMaxPeers);
-  const PeerRegionLayout L = peer_region_layout(tp, e->cfg.hidden);
-  {
-    cudaError_t er = cudaMalloc(&e->peer_region, L.total);
-    if (er != cudaSuccess) return fail(LSK_ERR_NOMEM, "cudaMalloc(peer region, %zu) failed: %s", L.total, cudaGetErrorString(er));
-  }
-  CU(cudaMemset(e->peer_region, 0, L.total));
+  TRY(e->mem.alloc(&e->peer_region, e->sizes.peer_region, true));
   CU(cudaDeviceSynchronize());
   cudaIpcMemHandle_t mine;
   CU(cudaIpcGetMemHandle(&mine, e->peer_region));
   const size_t hb = sizeof(cudaIpcMemHandle_t);
+  DeviceMem handles;                   // every rank's handle, on the device for the all-gather
   unsigned char* d_h = nullptr;
-  CU(cudaMalloc((void**)&d_h, hb * tp));
+  TRY(handles.alloc(&d_h, {hb * tp, MEM_SCRATCH}));
   CU(cudaMemcpy(d_h + hb * rank, &mine, hb, cudaMemcpyHostToDevice));
   NC(ncclAllGather(d_h + hb * rank, d_h, hb, ncclUint8, e->comm, e->stream));
   CU(cudaStreamSynchronize(e->stream));
   std::vector<cudaIpcMemHandle_t> all(tp);
   CU(cudaMemcpy(all.data(), d_h, hb * tp, cudaMemcpyDeviceToHost));
-  cudaFree(d_h);
   int local_ok = 1;
   std::string why;
   for (int r = 0; r < tp; ++r) {
@@ -1608,12 +1821,12 @@ int lsk_begin(lsk_engine* e, const lsk_generation* gen) {
   if (gen->sample) {
     if (!(gen->temperature > 0.f)) return fail(LSK_ERR_INVALID, "temperature must be > 0");
     TRY(ensure_logits(e));
-    TRY(alloc_once(&e->probs_d, (size_t)kMaxRows * e->cfg.vocab * 4));
-    TRY(alloc_once(&e->probs_v, (size_t)kMaxRows * e->cfg.vocab * 4));
-    TRY(alloc_once(&e->samp_scratch, (size_t)e->cfg.vocab * 4));
+    TRY(alloc_once(e, &e->probs_d, e->sizes.vocab_rows));
+    TRY(alloc_once(e, &e->probs_v, e->sizes.vocab_rows));
+    TRY(alloc_once(e, &e->samp_scratch, e->sizes.samp_scratch));
     if (e->cfg.tp_size > 1) {
-      TRY(alloc_once(&e->logits_gath, (size_t)e->cfg.tp_size * kMaxRows * e->vocab_l_pad * 4));
-      TRY(alloc_once(&e->logits_full, (size_t)kMaxRows * e->cfg.vocab * 4));
+      TRY(alloc_once(e, &e->logits_gath, e->sizes.logits_gath));
+      TRY(alloc_once(e, &e->logits_full, e->sizes.vocab_rows));
     }
   }
   e->gen = *gen;
@@ -1701,10 +1914,7 @@ int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_r
     if (drv < 12040) return fail(LSK_ERR_CUDA, "adaptive rounds need CUDA graph conditional nodes (driver >= 12.4, found %d)", drv);
     CU(cudaStreamCreateWithFlags(&e->body_stream, cudaStreamNonBlocking));
   }
-  if (!e->conf_scratch) {
-    CU(cudaMalloc((void**)&e->conf_scratch, sizeof(ConfScratch)));
-    CU(cudaMemsetAsync(e->conf_scratch, 0, sizeof(ConfScratch), e->stream));
-  }
+  TRY(alloc_once(e, &e->conf_scratch, e->sizes.conf_scratch, true));
   TRY(ensure_logits(e));                  // greedy drafts materialise their logits row
   // the threshold is read from device memory: one graph per round shape serves every threshold
   CU(cudaMemcpyAsync(&e->state->min_conf, &min_confidence, sizeof(float), cudaMemcpyHostToDevice, e->stream));
@@ -1803,19 +2013,18 @@ int lsk_debug_forward_rows(lsk_engine* e, const int32_t* ids, int32_t m) {
 // Scoring buffers, allocated on first use: the logits rows, result rows for k exits (regrown when a
 // call asks for more), and with `batch` packed scoring's group upload, arrival counters and view table.
 static int alloc_scoring(lsk_engine* e, int k, bool batch) {
-  const size_t P = (size_t)e->max_pos;
+  const MemTable& t = e->sizes;
   TRY(ensure_logits(e));
   if (k > e->score_cap) {
     e->score_cap = 0;
-    TRY(realloc_grown(&e->score_lp, (size_t)k * P * 4));
-    TRY(realloc_grown(&e->score_greedy, (size_t)k * P * 4));
+    TRY(realloc_grown(e, &e->score_lp, times(t.score_rows, k)));
+    TRY(realloc_grown(e, &e->score_greedy, times(t.score_rows, k)));
     e->score_cap = k;
   }
-  if (batch && !e->piece_arrive) {
-    TRY(alloc_once(&e->batch_buf, 8 * P * 4));
-    TRY(alloc_once(&e->view_table, P * 4));
-    TRY(alloc_once(&e->piece_arrive, (size_t)kPfTokens * e->kv_heads_l * 4));
-    CU(cudaMemsetAsync(e->piece_arrive, 0, (size_t)kPfTokens * e->kv_heads_l * 4, e->stream));
+  if (batch) {
+    TRY(alloc_once(e, &e->batch_buf, t.batch_buf));
+    TRY(alloc_once(e, &e->view_table, t.view_table));
+    TRY(alloc_once(e, &e->piece_arrive, t.piece_arrive, true));
   }
   return LSK_OK;
 }
@@ -1824,11 +2033,11 @@ static int alloc_scoring(lsk_engine* e, int k, bool batch) {
 // rows of a chunk, plus the warped full-depth rows of a slice.  A call with more exits regrows them.
 static int alloc_accept(lsk_engine* e, int k) {
   if (k - 1 <= e->accept_cap) return LSK_OK;
-  const size_t V = (size_t)e->cfg.vocab, P = (size_t)e->max_pos, rows = e->pf_tc ? kPfTokens : kMaxRows;
+  const MemTable& t = e->sizes;
   e->accept_cap = 0;
-  TRY(realloc_grown(&e->exits_accept, (size_t)(k - 1) * P * 4));
-  TRY(realloc_grown(&e->exits_pd, (size_t)(k - 1) * rows * V * 4));
-  TRY(alloc_once(&e->exits_pv, (size_t)kMaxRows * V * 4));
+  TRY(realloc_grown(e, &e->exits_accept, times(t.accept_rows, k - 1)));
+  TRY(realloc_grown(e, &e->exits_pd, times(t.draft_rows, k - 1)));
+  TRY(alloc_once(e, &e->exits_pv, t.vocab_rows));
   e->accept_cap = k - 1;
   return LSK_OK;
 }
@@ -1858,7 +2067,7 @@ static int score_sequence(lsk_engine* e, const int32_t* ids, int n, const int32_
   TRY(alloc_scoring(e, k, false));
   if (accept_out) TRY(alloc_accept(e, k));
   const int rows = n - 1, V = e->cfg.vocab;
-  const size_t P = (size_t)e->max_pos, pd_stride = (size_t)(e->pf_tc ? kPfTokens : kMaxRows) * V;
+  const size_t P = (size_t)e->max_pos, pd_stride = e->sizes.draft_rows.bytes / 4;   // floats per draft exit
   const WarpParams wp = accept_out ? WarpParams{sampling->temperature, sampling->top_k, sampling->top_p}
                                    : WarpParams{1.f, 0, 1.f};
   e->prefilled = false;
@@ -2406,43 +2615,42 @@ int lsk_test_pack(const void* w, int64_t n, int64_t k, void* packed) {
   return LSK_OK;
 }
 
+// The launch plumbing of an engine for one stand-alone test call: the SM count and a stream for
+// launches and zero fills.  The engine's destructor releases the stream, the events and every buffer
+// on every return path.
+static int test_engine(lsk_engine& t) {
+  int dev = 0;
+  CU(cudaGetDevice(&dev));
+  CU(cudaDeviceGetAttribute(&t.sm_count, cudaDevAttrMultiProcessorCount, dev));
+  CU(cudaStreamCreateWithFlags(&t.stream, cudaStreamNonBlocking));
+  t.mem.stream = t.stream;
+  return LSK_OK;
+}
+
 int lsk_test_gemm(const void* packed, int64_t n, int64_t k, const void* x, int32_t m, float* y,
                   int32_t iters, float* avg_ms) {
   if (!packed || !x || !y || n % 16 || k % 32 || m < 1 || m > kMaxRows) return fail(LSK_ERR_INVALID, "bad gemm test shape");
   lsk_engine tmp;   // only the launch plumbing is used
-  int dev = 0;
-  CU(cudaGetDevice(&dev));
-  CU(cudaDeviceGetAttribute(&tmp.sm_count, cudaDevAttrMultiProcessorCount, dev));
-  CU(cudaStreamCreateWithFlags(&tmp.stream, cudaStreamNonBlocking));
-  tmp.use_pdl = true;
+  TRY(test_engine(tmp));
   GemmPlan p = make_plan((int)n, (int)k);
   GemmArgs a{};
   a.W = (const uint4*)packed;
   a.M = m;
   a.x_bf16 = (const __nv_bfloat16*)x; a.xb_ld = (int)k;
   a.out_f32 = y; a.out_ld = (int)n;
-  cudaEvent_t e0, e1;
-  CU(cudaEventCreate(&e0));
-  CU(cudaEventCreate(&e1));
-  int st = launch_gemm<PRO_BF16, EPI_STORE>(&tmp, p, a);   // warm-up + result
-  if (st != LSK_OK) return st;
+  CU(cudaEventCreate(&tmp.ev0));
+  CU(cudaEventCreate(&tmp.ev1));
+  TRY((launch_gemm<PRO_BF16, EPI_STORE>(&tmp, p, a)));   // warm-up + result
   CU(cudaStreamSynchronize(tmp.stream));
   if (iters > 0) {
-    CU(cudaEventRecord(e0, tmp.stream));
-    for (int i = 0; i < iters; ++i) {
-      st = launch_gemm<PRO_BF16, EPI_STORE>(&tmp, p, a);
-      if (st != LSK_OK) return st;
-    }
-    CU(cudaEventRecord(e1, tmp.stream));
-    CU(cudaEventSynchronize(e1));
+    CU(cudaEventRecord(tmp.ev0, tmp.stream));
+    for (int i = 0; i < iters; ++i) TRY((launch_gemm<PRO_BF16, EPI_STORE>(&tmp, p, a)));
+    CU(cudaEventRecord(tmp.ev1, tmp.stream));
+    CU(cudaEventSynchronize(tmp.ev1));
     float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, e0, e1));
+    CU(cudaEventElapsedTime(&ms, tmp.ev0, tmp.ev1));
     if (avg_ms) *avg_ms = ms / iters;
   }
-  CU(cudaEventDestroy(e0));
-  CU(cudaEventDestroy(e1));
-  CU(cudaStreamDestroy(tmp.stream));
-  tmp.stream = nullptr;
   return LSK_OK;
 }
 
@@ -2486,81 +2694,56 @@ int lsk_test_attn(const void* q, const void* k, const void* v, int32_t n_heads, 
     return fail(LSK_ERR_INVALID, "bad attention test shape");
   const bool prompt = m > kMaxRows;
   lsk_engine tmp;
-  // every buffer, event and the stream are released on every return path (errors included)
-  struct Owned {
-    lsk_engine& t;
-    __nv_bfloat16 *kp = nullptr, *vp = nullptr;
-    int *pt = nullptr, *len = nullptr;
-    unsigned char* canon = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    ~Owned() {
-      if (t.stream) cudaStreamSynchronize(t.stream);
-      void* bufs[] = {kp, vp, pt, len, canon, t.attn_part, t.attn_arrive};
-      for (void* b : bufs) if (b) cudaFree(b);
-      if (e0) cudaEventDestroy(e0);
-      if (e1) cudaEventDestroy(e1);
-      if (t.stream) cudaStreamDestroy(t.stream);
-      t.stream = nullptr;
-    }
-  } o{tmp};
-  {
-    int dev = 0;
-    CU(cudaGetDevice(&dev));
-    CU(cudaDeviceGetAttribute(&tmp.sm_count, cudaDevAttrMultiProcessorCount, dev));
-  }
-  CU(cudaStreamCreateWithFlags(&tmp.stream, cudaStreamNonBlocking));
-  tmp.use_pdl = true;
+  TRY(test_engine(tmp));
   tmp.n_splits = n_splits;
-  TRY(alloc_attn_partials(&tmp, n_kv_heads, n_heads / n_kv_heads, head_dim, m));
+  TRY(alloc_attn_partials(&tmp, attn_bufs(n_kv_heads, n_heads / n_kv_heads, head_dim, n_splits, m)));
   const int n_pages = (ctx + kPageTokens - 1) / kPageTokens;
   const size_t pool_elems = (size_t)n_pages * n_kv_heads * kPageTokens * kHeadDim;
   std::vector<int> pth(n_pages);
   for (int i = 0; i < n_pages; ++i) pth[i] = page_perm ? page_perm[i] : i;
   for (int i = 0; i < n_pages; ++i)
     if (pth[i] < 0 || pth[i] >= n_pages) return fail(LSK_ERR_INVALID, "bad page permutation");
-  CU(cudaMalloc((void**)&o.kp, pool_elems * 2));
-  CU(cudaMalloc((void**)&o.vp, pool_elems * 2));
-  CU(cudaMalloc((void**)&o.pt, (size_t)n_pages * 4));
-  CU(cudaMalloc((void**)&o.len, 4));
-  CU(cudaMemsetAsync(o.kp, 0, pool_elems * 2, tmp.stream));
-  CU(cudaMemsetAsync(o.vp, 0, pool_elems * 2, tmp.stream));
+  __nv_bfloat16 *kp = nullptr, *vp = nullptr;
+  int *pt = nullptr, *len = nullptr;
+  unsigned char* canon = nullptr;
+  TRY(tmp.mem.alloc(&kp, {pool_elems * 2, MEM_KV_POOL}, true));
+  TRY(tmp.mem.alloc(&vp, {pool_elems * 2, MEM_KV_POOL}, true));
+  TRY(tmp.mem.alloc(&pt, {(size_t)n_pages * 4, MEM_SCRATCH}));
+  TRY(tmp.mem.alloc(&len, {4, MEM_SCRATCH}));
   const int base = prompt ? 0 : ctx - m;
   const int q_cols = n_heads * kHeadDim;
-  if (prompt) {
-    CU(cudaMalloc((void**)&o.canon, (size_t)((q_cols + 63) / 64) * kCanonStageBytes));
-    CU(cudaMemsetAsync(o.canon, 0, (size_t)((q_cols + 63) / 64) * kCanonStageBytes, tmp.stream));
-  }
-  CU(cudaMemcpyAsync(o.pt, pth.data(), (size_t)n_pages * 4, cudaMemcpyHostToDevice, tmp.stream));
-  CU(cudaMemcpyAsync(o.len, &base, 4, cudaMemcpyHostToDevice, tmp.stream));
-  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)k, n_kv_heads, ctx, head_dim, o.pt, o.kp);
-  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)v, n_kv_heads, ctx, head_dim, o.pt, o.vp);
+  if (prompt) TRY(tmp.mem.alloc(&canon, {(size_t)((q_cols + 63) / 64) * kCanonStageBytes, MEM_SCRATCH}, true));
+  CU(cudaMemcpyAsync(pt, pth.data(), (size_t)n_pages * 4, cudaMemcpyHostToDevice, tmp.stream));
+  CU(cudaMemcpyAsync(len, &base, 4, cudaMemcpyHostToDevice, tmp.stream));
+  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)k, n_kv_heads, ctx, head_dim, pt, kp);
+  paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)v, n_kv_heads, ctx, head_dim, pt, vp);
   CU(cudaGetLastError());
   AttnArgs a{};
   a.q = (const __nv_bfloat16*)q; a.q_ld = q_cols;
   a.out = (__nv_bfloat16*)out; a.out_ld = q_cols;
-  a.kpool = o.kp; a.vpool = o.vp; a.page_table = o.pt; a.base_len = o.len; a.pos_off = 0; a.M = m;
+  a.kpool = kp; a.vpool = vp; a.page_table = pt; a.base_len = len; a.pos_off = 0; a.M = m;
   a.group = n_heads / n_kv_heads; a.n_kv_heads = n_kv_heads; a.n_splits = n_splits;
   a.scale = 1.0f / sqrtf((float)kHeadDim);
   auto run = [&]() -> int {
     if (!prompt) return launch_attention(&tmp, a, head_dim);
-    return launch_prompt_attention(&tmp, (const __nv_bfloat16*)q, q_cols, o.canon, o.kp, o.vp, o.pt, o.len, ctx - m, m,
+    return launch_prompt_attention(&tmp, (const __nv_bfloat16*)q, q_cols, canon, kp, vp, pt, len, ctx - m, m,
                                    n_heads / n_kv_heads, n_kv_heads, head_dim);
   };
   TRY(run());
   if (prompt) {
-    uncanon_rows_kernel<<<tmp.sm_count, 256, 0, tmp.stream>>>(o.canon, m, q_cols, (__nv_bfloat16*)out);
+    uncanon_rows_kernel<<<tmp.sm_count, 256, 0, tmp.stream>>>(canon, m, q_cols, (__nv_bfloat16*)out);
     CU(cudaGetLastError());
   }
   CU(cudaStreamSynchronize(tmp.stream));
   if (iters > 0) {
-    CU(cudaEventCreate(&o.e0));
-    CU(cudaEventCreate(&o.e1));
-    CU(cudaEventRecord(o.e0, tmp.stream));
+    CU(cudaEventCreate(&tmp.ev0));
+    CU(cudaEventCreate(&tmp.ev1));
+    CU(cudaEventRecord(tmp.ev0, tmp.stream));
     for (int i = 0; i < iters; ++i) TRY(run());
-    CU(cudaEventRecord(o.e1, tmp.stream));
-    CU(cudaEventSynchronize(o.e1));
+    CU(cudaEventRecord(tmp.ev1, tmp.stream));
+    CU(cudaEventSynchronize(tmp.ev1));
     float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, o.e0, o.e1));
+    CU(cudaEventElapsedTime(&ms, tmp.ev0, tmp.ev1));
     if (avg_ms) *avg_ms = ms / iters;
   }
   return LSK_OK;
@@ -2575,6 +2758,7 @@ int lsk_test_lmhead_tc(const void* w, int64_t n, int64_t k, const float* x, cons
   int stages = kTcMaxStages;
   while (stages >= 3 && lmhead_tc_smem_bytes((int)k, stages) > (size_t)kSmemMax) --stages;
   if (stages < 3) return fail(LSK_ERR_INVALID, "hidden %lld does not fit the wgmma LM head", (long long)k);
+  lsk_engine tmp;   // holds the buffers and events; the kernels run on the legacy default stream
   int dev = 0, sms = 0;
   CU(cudaGetDevice(&dev));
   CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -2584,9 +2768,9 @@ int lsk_test_lmhead_tc(const void* w, int64_t n, int64_t k, const float* x, cons
   unsigned char* canon = nullptr;
   float* cval = nullptr;
   int* cidx = nullptr;
-  CU(cudaMalloc((void**)&canon, (size_t)n_tiles * kTcTileRows * k * 2));
-  CU(cudaMalloc((void**)&cval, (size_t)grid * kMaxRows * 4));
-  CU(cudaMalloc((void**)&cidx, (size_t)grid * kMaxRows * 4));
+  TRY(tmp.mem.alloc(&canon, {(size_t)n_tiles * kTcTileRows * k * 2, MEM_LM_HEAD}));
+  TRY(tmp.mem.alloc(&cval, {(size_t)grid * kMaxRows * 4, MEM_SCRATCH}));
+  TRY(tmp.mem.alloc(&cidx, {(size_t)grid * kMaxRows * 4, MEM_SCRATCH}));
   pack_canonical_kernel<<<sms * 8, 256>>>((const __nv_bfloat16*)w, k, 0, n, k, reinterpret_cast<uint4*>(canon), n_tiles);
   CU(cudaGetLastError());
   CU(cudaFuncSetAttribute(lmhead_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax));
@@ -2596,26 +2780,22 @@ int lsk_test_lmhead_tc(const void* w, int64_t n, int64_t k, const float* x, cons
   t.logits = logits; t.logits_ld = (int)n; t.n_valid_rows = (int)n; t.vocab_off = 0;
   t.part_val = cval; t.part_idx = cidx;
   const size_t smem = lmhead_tc_smem_bytes((int)k, stages);
-  cudaEvent_t e0, e1;
-  CU(cudaEventCreate(&e0));
-  CU(cudaEventCreate(&e1));
+  CU(cudaEventCreate(&tmp.ev0));
+  CU(cudaEventCreate(&tmp.ev1));
   lmhead_tc_kernel<<<grid, kTcThreads, smem>>>(t);
   CU(cudaGetLastError());
   rank_best_kernel<<<1, 256>>>(cval, cidx, grid, m, best_val, best_idx);
   CU(cudaGetLastError());
   CU(cudaDeviceSynchronize());
   if (iters > 0) {
-    CU(cudaEventRecord(e0));
+    CU(cudaEventRecord(tmp.ev0));
     for (int i = 0; i < iters; ++i) lmhead_tc_kernel<<<grid, kTcThreads, smem>>>(t);
-    CU(cudaEventRecord(e1));
-    CU(cudaEventSynchronize(e1));
+    CU(cudaEventRecord(tmp.ev1));
+    CU(cudaEventSynchronize(tmp.ev1));
     float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, e0, e1));
+    CU(cudaEventElapsedTime(&ms, tmp.ev0, tmp.ev1));
     if (avg_ms) *avg_ms = ms / iters;
   }
-  CU(cudaEventDestroy(e0));
-  CU(cudaEventDestroy(e1));
-  cudaFree(canon); cudaFree(cval); cudaFree(cidx);
   return LSK_OK;
 }
 
@@ -2638,34 +2818,18 @@ int lsk_test_accept(const float* logits_draft, const float* logits_verify, int32
     return fail(LSK_ERR_INVALID, "bad acceptance test shape");
   if (!(sampling->temperature > 0.f)) return fail(LSK_ERR_INVALID, "acceptance test needs temperature > 0");
   const WarpParams wp{sampling->temperature, sampling->top_k, sampling->top_p};
+  DeviceMem mem;
   float* buf = nullptr;
-  CU(cudaMalloc((void**)&buf, (size_t)2 * rows * vocab * 4));
+  TRY(mem.alloc(&buf, {(size_t)2 * rows * vocab * 4, MEM_SCRATCH}));
   warp_rows_kernel<<<rows, kSampleThreads>>>(logits_draft, ld, vocab, wp, buf);
   accept_prob_kernel<<<rows, kSampleThreads>>>(logits_verify, ld, vocab, wp, buf, (size_t)0, 1,
                                                buf + (size_t)rows * vocab, accept, (size_t)0);
-  const cudaError_t er = cudaGetLastError();
-  const cudaError_t es = cudaDeviceSynchronize();
-  cudaFree(buf);
-  CU(er);
-  CU(es);
+  CU(cudaGetLastError());
+  CU(cudaDeviceSynchronize());
   return LSK_OK;
 }
 
 }  // extern "C"
-
-// device buffers of one stand-alone sampling test call, released when it returns
-struct TestBuffers {
-  std::vector<void*> ptrs;
-  ~TestBuffers() {
-    for (void* p : ptrs) cudaFree(p);
-  }
-  template <typename T>
-  cudaError_t alloc(T** out, size_t count) {
-    const cudaError_t er = cudaMalloc((void**)out, std::max<size_t>(count, 1) * sizeof(T));
-    if (er == cudaSuccess) ptrs.push_back(*out);
-    return er;
-  }
-};
 
 static GenParams gen_params_of(const lsk_generation& g) {
   GenParams gp{};
@@ -2703,13 +2867,13 @@ int lsk_test_sample(const float* logits, int32_t rows, int32_t vocab, int32_t ld
     states[s] = DevState{};
     states[s].step_count = step0 + s;
   }
-  TestBuffers bufs;
+  DeviceMem mem;
   GenParams* gp_dev = nullptr;
   DevState* st_dev = nullptr;
   float* later = nullptr;                // the warped rows of steps > 0 (the same values again)
-  CU(bufs.alloc(&gp_dev, 1));
-  CU(bufs.alloc(&st_dev, (size_t)n_steps));
-  if (n_steps > 1) CU(bufs.alloc(&later, (size_t)rows * vocab));
+  TRY(mem.alloc(&gp_dev, {sizeof(GenParams), MEM_SCRATCH}));
+  TRY(mem.alloc(&st_dev, {(size_t)n_steps * sizeof(DevState), MEM_SCRATCH}));
+  if (n_steps > 1) TRY(mem.alloc(&later, {(size_t)rows * vocab * 4, MEM_SCRATCH}));
   CU(cudaMemcpy(gp_dev, &gp, sizeof(gp), cudaMemcpyHostToDevice));
   CU(cudaMemcpy(st_dev, states.data(), states.size() * sizeof(DevState), cudaMemcpyHostToDevice));
   for (int s = 0; s < n_steps; ++s)
@@ -2740,13 +2904,13 @@ int lsk_test_accept_sample(const float* p_draft, const float* p_verify, int32_t 
     for (int i = 0; i < d; ++i) st.tok[1 + i] = draft_ids[(size_t)s * d + i];
     for (int i = 0; i <= d; ++i) st.verified[i] = verified_ids[(size_t)s * (d + 1) + i];
   }
-  TestBuffers bufs;
+  DeviceMem mem;
   GenParams* gp_dev = nullptr;
   DevState* st_dev = nullptr;
   RoundResult* res_dev = nullptr;
-  CU(bufs.alloc(&gp_dev, 1));
-  CU(bufs.alloc(&st_dev, (size_t)n_steps));
-  CU(bufs.alloc(&res_dev, (size_t)n_steps));
+  TRY(mem.alloc(&gp_dev, {sizeof(GenParams), MEM_SCRATCH}));
+  TRY(mem.alloc(&st_dev, {(size_t)n_steps * sizeof(DevState), MEM_SCRATCH}));
+  TRY(mem.alloc(&res_dev, {(size_t)n_steps * sizeof(RoundResult), MEM_SCRATCH}));
   CU(cudaMemcpy(gp_dev, &gp, sizeof(gp), cudaMemcpyHostToDevice));
   CU(cudaMemcpy(st_dev, states.data(), states.size() * sizeof(DevState), cudaMemcpyHostToDevice));
   CU(cudaMemset(res_dev, 0, (size_t)n_steps * sizeof(RoundResult)));

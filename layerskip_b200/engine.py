@@ -14,7 +14,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 import torch
 
 from . import _lib
-from .weights import ROPE_KINDS, LlamaArch, SyntheticLlama, iter_state_dict
+from .weights import LlamaArch, SyntheticLlama, iter_state_dict
 
 
 @dataclass
@@ -41,6 +41,8 @@ class Engine:
         self.device = torch.device(device) if device is not None else \
             torch.device("cuda", torch.cuda.current_device())
         self.tp_rank, self.tp_size = tp_rank, tp_size
+        # the memory plan counts per-SM buffers: asked only when there is free memory to plan against
+        sm_count = lambda: torch.cuda.get_device_properties(self.device).multi_processor_count  # noqa: E731
         # the tensor-core prompt pass needs a second (canonical-layout) copy of the layer weights: on by
         # default, dropped automatically when the two copies would not fit this GPU
         try:
@@ -52,7 +54,7 @@ class Engine:
             if prefill_tc and free_now is not None:
                 from .memory import plan_memory
                 plan = plan_memory(arch, max_ctx=max_ctx, tp_size=tp_size, keep_logits=keep_logits,
-                                   prefill_tc=True)
+                                   prefill_tc=True, sm_count=sm_count())
                 if plan["total"] + plan["weights_source_peak"] > free_now:
                     prefill_tc = False
         self.prefill_tc = bool(prefill_tc)
@@ -60,15 +62,7 @@ class Engine:
                 (0 if prefill_tc else _lib.LSK_FLAG_NO_PREFILL_TC) | \
                 (0 if use_pdl else _lib.LSK_FLAG_NO_PDL) | (0 if use_graph else _lib.LSK_FLAG_NO_GRAPH) | \
                 (_lib.LSK_FLAG_TP_NCCL if tp_nccl else 0)
-        cfg = _lib.lsk_config(
-            vocab=arch.vocab, hidden=arch.hidden, inter=arch.inter, n_layers=arch.layers,
-            n_heads=arch.heads, n_kv_heads=arch.kv_heads, head_dim=arch.head_dim,
-            rms_eps=arch.rms_eps, rope_theta=arch.rope_theta, max_ctx=max_ctx, tp_rank=tp_rank,
-            tp_size=tp_size, attn_splits=attn_splits, flags=flags,
-            rope_scaling=ROPE_KINDS[arch.rope_scaling], rope_factor=arch.rope_factor,
-            rope_low_freq_factor=arch.rope_low_freq_factor,
-            rope_high_freq_factor=arch.rope_high_freq_factor,
-            rope_original_max_pos=arch.rope_original_max_pos)
+        cfg = arch.lsk_config(max_ctx, tp_rank=tp_rank, tp_size=tp_size, attn_splits=attn_splits, flags=flags)
         self.max_ctx = max_ctx
         self.keep_logits = keep_logits
         # refuse a configuration that cannot fit BEFORE cudaMalloc fails half-way (memory.py)
@@ -80,7 +74,7 @@ class Engine:
             from .memory import check_fits
             check_fits(arch, free_bytes, max_ctx=max_ctx, tp_size=tp_size, keep_logits=keep_logits,
                        sampling=False, lm_head_tc=os.environ.get("LSK_LMHEAD_TC", "0") not in ("", "0"),
-                       prefill_tc=self.prefill_tc)
+                       prefill_tc=self.prefill_tc, sm_count=sm_count())
         handle = C.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(self._lib.lsk_create(C.byref(cfg), C.byref(handle)))
@@ -91,8 +85,7 @@ class Engine:
         # K-chunked normalisation above), else 8
         plan = _lib.lsk_gemm_plan()
         qkv_rows = (arch.heads + 2 * arch.kv_heads) // tp_size * arch.head_dim
-        sms = torch.cuda.get_device_properties(self.device).multi_processor_count
-        ok = self._lib.lsk_plan_gemm((qkv_rows + 15) // 16 * 16, arch.hidden, 16, 0, 0, sms, C.byref(plan))
+        ok = self._lib.lsk_plan_gemm((qkv_rows + 15) // 16 * 16, arch.hidden, 16, 0, 0, sm_count(), C.byref(plan))
         self.max_rows = 16 if (ok == 0 and plan.ok) else 8
 
     # ------------------------------------------------------------------ lifetime

@@ -98,6 +98,19 @@ class LlamaArch:
                      original_max_position_embeddings=self.rope_original_max_pos)
         return d
 
+    def lsk_config(self, max_ctx: int, tp_rank: int = 0, tp_size: int = 1, attn_splits: int = 0,
+                   flags: int = 0) -> "_lib.lsk_config":
+        """The engine config (`lsk_config`) of this architecture."""
+        return _lib.lsk_config(
+            vocab=self.vocab, hidden=self.hidden, inter=self.inter, n_layers=self.layers,
+            n_heads=self.heads, n_kv_heads=self.kv_heads, head_dim=self.head_dim,
+            rms_eps=self.rms_eps, rope_theta=self.rope_theta, max_ctx=max_ctx, tp_rank=tp_rank,
+            tp_size=tp_size, attn_splits=attn_splits, flags=flags,
+            rope_scaling=ROPE_KINDS[self.rope_scaling], rope_factor=self.rope_factor,
+            rope_low_freq_factor=self.rope_low_freq_factor,
+            rope_high_freq_factor=self.rope_high_freq_factor,
+            rope_original_max_pos=self.rope_original_max_pos)
+
     @property
     def q_dim(self) -> int:
         return self.heads * self.head_dim

@@ -85,6 +85,8 @@ def test_engine_raises_before_it_allocates(monkeypatch):
     from layerskip_b200.engine import Engine
     monkeypatch.setattr(torch.cuda, "is_available", lambda: True)
     monkeypatch.setattr(torch.cuda, "mem_get_info", lambda *a: (_ for _ in ()).throw(RuntimeError("no query")))
+    monkeypatch.setattr(torch.cuda, "get_device_properties",
+                        lambda *a: type("Props", (), dict(multi_processor_count=132))())
     monkeypatch.setattr(torch.cuda, "device", lambda *a: contextlib.nullcontext())
     arch = LlamaArch(512, 4096, 11008, 2, 32, 1, 128)
     with pytest.raises(_lib.LskError, match="group 32"):
