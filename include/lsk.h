@@ -164,6 +164,32 @@ int lsk_round(lsk_engine* e, int32_t d_req, lsk_round_out* out);
 int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_round_out* out,
                        float* draft_conf_out);
 
+/* Batched greedy generation: n_seqs prompts share every weight pass of a round.  The batch shares
+ * the KV pool: sequence s owns a slot of P = n_pages / n_seqs whole 64-token pages, logical pages
+ * [s*P, (s+1)*P), and its position p is logical position s*64*P + p (LSK_DBG_KROW / LSK_DBG_VROW
+ * read it there).  Every active sequence's round and the state it leaves are bit-identical to
+ * lsk_round(e, d_seq[s]) run on that sequence alone (lsk_begin + lsk_prefill of its prompt, then the
+ * same earlier rounds).  After lsk_begin with sample == 0, no_repeat_ngram_size == 0, tp_size == 1 and
+ * 1 <= exit_layer <= n_layers; n_seqs in [1, max_rows].
+ *
+ * lsk_prefill_batch: prompt j is ids[offsets[j] .. offsets[j+1]-1] (offsets[0] == 0), length >= 1;
+ * each is prefilled into its own slot exactly as lsk_prefill would prefill it alone (same routes,
+ * same bits).  slot_positions_out (may be NULL): positions per slot, 64 * P.  LSK_ERR_CTX when a
+ * prompt + 1 does not fit its slot.  Ends any single-sequence generation: lsk_round,
+ * lsk_round_adaptive and lsk_ar_step return LSK_ERR_STATE until the next lsk_prefill.
+ *
+ * lsk_round_batch: one round for every sequence, n_seqs * (d_req + 1) <= max_rows.  d_seq (may be NULL:
+ * all d_req) holds each sequence's draft count in [0, d_req]; active (may be NULL: all active) flags
+ * the sequences that commit.  An inactive sequence commits nothing: outs[s] has n_drafted = n_matches
+ * = n_emitted = 0 and kv_len unchanged (its rows still run, writing K/V only inside its own slot above
+ * its committed length).  LSK_ERR_CTX when some sequence, active or not, has kv_len + d_req + 2 above
+ * its slot's positions; LSK_ERR_STATE after any lsk_prefill or scoring call since the batch's
+ * prefill.  outs: n_seqs records. */
+int lsk_prefill_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
+                      int32_t* slot_positions_out);
+int lsk_round_batch(lsk_engine* e, int32_t d_req, const int32_t* d_seq, const int32_t* active,
+                    lsk_round_out* outs);
+
 /* One autoregressive step on the same engine (autoregressive_generator.py:44-67): all layers, or
  * layers < E when the generation's exit_layer > 0.  Returns the chosen token; the caller decides
  * about EOS exactly as the reference does (:66-67). */
@@ -306,6 +332,8 @@ typedef struct {
   int32_t accept_exits;      /* lsk_score_exits with accept_out, up to this many exits            */
   int32_t packed_scoring;    /* lsk_score_batch or lsk_score_prefixed                             */
   int32_t tp_peer;           /* tp_size > 1: lsk_comm_init's peer region of the one-shot collectives */
+  int32_t batch_seqs;        /* lsk_prefill_batch with up to this many sequences, <= 16 (any count
+                              * allocates the same buffers)                                      */
 } lsk_memory_uses;
 /* Host-side plan of the device memory an engine with config `cfg` on a GPU with `sm_count` SMs
  * allocates at lsk_create plus for `uses` (pure host logic; works without a GPU).  The flags it

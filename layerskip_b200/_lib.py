@@ -89,7 +89,7 @@ class lsk_memory_plan(C.Structure):
 class lsk_memory_uses(C.Structure):
     _fields_ = [("lm_head_tc", C.c_int32), ("sampling", C.c_int32), ("ngram_ban", C.c_int32),
                 ("adaptive", C.c_int32), ("score_exits", C.c_int32), ("accept_exits", C.c_int32),
-                ("packed_scoring", C.c_int32), ("tp_peer", C.c_int32)]
+                ("packed_scoring", C.c_int32), ("tp_peer", C.c_int32), ("batch_seqs", C.c_int32)]
 
 
 # name -> (restype, argtypes); every symbol include/lsk.h declares
@@ -107,6 +107,10 @@ SIGNATURES = {
     "lsk_round": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(lsk_round_out)]),
     "lsk_round_adaptive": (C.c_int, [C.c_void_p, C.c_int32, C.c_float, C.POINTER(lsk_round_out),
                                      C.POINTER(C.c_float)]),
+    "lsk_prefill_batch": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                    C.POINTER(C.c_int32)]),
+    "lsk_round_batch": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                  C.POINTER(lsk_round_out)]),
     "lsk_ar_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "lsk_score": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32,
                             C.POINTER(C.c_float), C.POINTER(C.c_int32)]),

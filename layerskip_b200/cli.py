@@ -40,6 +40,9 @@ class BenchmarkArguments:             # benchmark.py:43-50
     n_shot: Optional[int] = 0
     template: Optional[str] = None
     prompt_len: int = 128             # synthetic dataset only
+    # not in the reference: generate the prompts this many at a time (greedy self-speculation only,
+    # B200SelfSpeculativeGenerationStrategy.generate_batch); 1 generates them one by one
+    batch_size: int = 1
 
 
 @dataclass
@@ -156,6 +159,8 @@ def benchmark(model, tokenizer, bench_args: BenchmarkArguments, gen_cfg: Generat
     # the reference times an already-loaded model: build the engine (weight upload / repack, CUDA
     # graph capture) and run one short generation BEFORE the timed loop
     warm = GenerationConfig(**{**vars(gen_cfg), "max_steps": min(8, gen_cfg.max_steps)})
+    if bench_args.batch_size > 1:
+        return _benchmark_batched(generator, examples, bench_args.batch_size, gen_cfg, warm, means)
     generator.generate(examples[0], warm)
     for prompt in examples:
         res: GenerationResult = generator.generate(prompt, gen_cfg)
@@ -164,6 +169,32 @@ def benchmark(model, tokenizer, bench_args: BenchmarkArguments, gen_cfg: Generat
         means["time_per_token"].update(res.time_per_token)
         means["tokens_per_second"].update(res.tokens_per_second)
     generator.generation_strategy.engines.close()
+    return {k: {"mean": v.compute()} for k, v in means.items()}
+
+
+def _benchmark_batched(generator, examples: List[str], batch_size: int, gen_cfg: GenerationConfig,
+                       warm: GenerationConfig, means: Dict[str, Mean]) -> Dict[str, Any]:
+    """`benchmark` with the prompts generated batch_size at a time (generate_batch).  Each prompt's
+    acceptance rate is its own; total time is the wall time of its group's generate_batch call, and
+    time per token / tokens per second count every token of the group over that time."""
+    strategy = generator.generation_strategy
+    if not hasattr(strategy, "generate_batch"):
+        raise ValueError("--batch_size > 1 needs --generation_strategy self_speculative")
+    tok = generator.tokenizer
+    eos_ids = list(gen_cfg.stop_token_ids) + [tok.eos_token_id]
+    ids = [tok(p, return_tensors="pt", add_special_tokens=True)["input_ids"].tolist()[0] for p in examples]
+    strategy.generate_batch(generator.model, ids[:batch_size], eos_ids, warm)
+    for g in range(0, len(ids), batch_size):
+        t0 = time.perf_counter()
+        results = strategy.generate_batch(generator.model, ids[g:g + batch_size], eos_ids, gen_cfg)
+        elapsed = time.perf_counter() - t0
+        n = sum(len(r.predicted_tokens) for r in results)
+        for r in results:
+            means["acceptance_rate"].update(r.acceptance_rate)
+            means["total_time"].update(elapsed)
+        means["time_per_token"].update(elapsed / n if n else None)
+        means["tokens_per_second"].update(n / elapsed)
+    strategy.engines.close()
     return {k: {"mean": v.compute()} for k, v in means.items()}
 
 

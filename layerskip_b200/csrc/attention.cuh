@@ -62,9 +62,13 @@ struct AttnArgs {
 // rows, position of that row, first logical page of its page-table view).  q, the canonical output
 // and the partials are addressed by chunk row; AttnArgs::M is the largest piece's rows,
 // AttnArgs::arrive holds [pieces][n_kv_heads] counters.
+// Sequence grid (batched rounds, pieces == nullptr): piece z is sequence z's seq_rows rows, chunk row
+// z * seq_rows, at position *(base_len + z * len_stride) + pos_off + i, over its page-table view
+// page_table + z * seq_pages.  Packed scoring's pieces all read *base_len (len_stride 0).
 struct AttnPieces {
   const int4* pieces;
-  int part_rows;               // row stride of AttnArgs::part: rows_pad of a whole 128-row chunk
+  int part_rows;               // row stride of AttnArgs::part: rows_pad of all the launch's rows
+  int seq_rows, len_stride, seq_pages;
 };
 
 // floats of AttnArgs::part for a launch
@@ -210,7 +214,10 @@ __device__ __forceinline__ void attn_split_body(const AttnArgs& a, const AttnPie
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
   // this CTA's query rows: the whole launch, or piece blockIdx.z (chunk row tok0)
-  const int4 pc = PIECES ? pz.pieces[blockIdx.z] : make_int4(0, 0, 0, 0);
+  const int z = blockIdx.z;
+  const int4 pc = !PIECES ? make_int4(0, 0, 0, 0)
+                  : pz.pieces ? pz.pieces[z] : make_int4(z * pz.seq_rows, pz.seq_rows, a.pos_off, z * pz.seq_pages);
+  const int* base_len = PIECES ? a.base_len + z * pz.len_stride : a.base_len;
   const int tok0 = pc.x;
   const int M = PIECES ? pc.y : a.M;
   const int pos_off = PIECES ? pc.z : a.pos_off;
@@ -226,7 +233,7 @@ __device__ __forceinline__ void attn_split_body(const AttnArgs& a, const AttnPie
 
   // ---- everything below up to pdl_wait() reads only data that is constant while the enclosing
   // graph runs: the committed length, the page table, and K/V rows below the committed length
-  const int len0 = *a.base_len;
+  const int len0 = *base_len;
   const int base = len0 + pos_off;                   // position of token row 0
   const int n_keys = base + M;                       // keys visible to the last row
   const int n_kgroups = (n_keys + kKeyGroup - 1) / kKeyGroup;
@@ -468,7 +475,8 @@ attn_split_kernel(const AttnArgs a) {
   attn_split_body<HD, false>(a, AttnPieces{nullptr, 0});
 }
 
-// grid (kv heads, splits, pieces): every piece of a packed prompt-pass chunk in one launch
+// grid (kv heads, splits, pieces): every piece of a packed prompt-pass chunk, or every sequence of a
+// batched round, in one launch
 template <int HD>
 __global__ void __launch_bounds__(kAttnThreads)
 attn_piece_kernel(const AttnArgs a, const AttnPieces pz) {

@@ -188,6 +188,7 @@ struct MemTable {
   MemBuf score_rows;      // per exit, each of score_lp, score_greedy
   MemBuf accept_rows, draft_rows;                   // per draft exit: exits_accept, exits_pd
   MemBuf batch_buf, view_table, piece_arrive;       // packed scoring
+  MemBuf batch_state, batch_ctl, batch_arrive;      // batched rounds
   MemBuf peer_region;                               // lsk_comm_init with the one-shot collectives
 };
 
@@ -258,6 +259,14 @@ struct lsk_engine : EngineShape {
   GenParams* gen_dev = nullptr;
   RoundResult* res_host = nullptr;     // mapped pinned
   RoundResult* res_dev = nullptr;      // device alias of res_host
+  // batched rounds (lsk_prefill_batch / lsk_round_batch; allocated on first use)
+  int batch_n = 0;                     // sequences of the batch in progress; 0: none
+  std::vector<int> batch_len;          // host mirror of each sequence's committed length
+  DevState* bstate = nullptr;          // [kMaxRows] per-sequence generation state
+  int* batch_ctl = nullptr;            // [2][kMaxRows] the round's d_seq, then its active flags
+  unsigned int* batch_arrive = nullptr;  // [kMaxRows][kv heads] attention arrival counters
+  RoundResult* bres_host = nullptr;    // [kMaxRows] mapped pinned
+  RoundResult* bres_dev = nullptr;     // device alias of bres_host
 
   GemmPlan p_qkv, p_o, p_gu, p_d, p_lm;
   const float* cur_cand_val = nullptr;  // candidates of the last enqueued LM head (epilogue's, or the banned rows' arg-max)
@@ -307,6 +316,7 @@ struct lsk_engine : EngineShape {
     mem.release();
     if (peer_err_host) cudaFreeHost(peer_err_host);
     if (res_host) cudaFreeHost(res_host);
+    if (bres_host) cudaFreeHost(bres_host);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (stream) cudaStreamDestroy(stream);
@@ -570,7 +580,8 @@ static int launch_attention_t(lsk_engine* e, AttnArgs& a, const AttnPieces* pz, 
   a.merge_off = sp.merge_off; a.part_off = sp.part_off; a.reload_per_rb = sp.reload_per_rb;
   if (attn_part_floats(a.n_kv_heads, a.n_splits, pz ? pz->part_rows : a.rows_pad, HD) > e->attn_part_cap)
     return fail(LSK_ERR_INVALID, "attention: %d query rows per kv head exceed the partials buffer", a.group * a.M);
-  a.part = e->attn_part; a.arrive = pz ? e->piece_arrive : e->attn_arrive;
+  // counters per (piece, kv head): packed scoring's pieces, or a batched round's sequences
+  a.part = e->attn_part; a.arrive = pz ? (pz->pieces ? e->piece_arrive : e->batch_arrive) : e->attn_arrive;
   // lp.smem: a grid that fits one wave gets a whole SM per CTA (> half of the SM's shared memory):
   // the CTAs then spread over the SMs instead of sharing a few SMs' load bandwidth
   const dim3 grid(a.n_kv_heads, a.n_splits, grid_z);
@@ -605,14 +616,25 @@ static int alloc_attn_partials(lsk_engine* e, const AttnBufs& b) {
   return e->mem.alloc(&e->attn_arrive, b.arrive, true);
 }
 
+// Rows of several sequences in one launch (batched rounds, single GPU): n_seqs sequences of seq_rows
+// rows each, sequence s's rows first at hidden row row0 + s * x_ld / hidden, its committed length at
+// base_len[s * len_stride] and its page-table view at page_table + s * seq_pages.  The activations
+// between the GEMMs (q, attention output, act) stay contiguous.
+struct SeqRows {
+  int n_seqs, seq_rows, len_stride, seq_pages, x_ld;
+};
+
 // ---------------------------------------------------------------------------------------------
 // one decoder layer on hidden rows [row0, row0 + M) at positions *base_len + pos_off + i
 //   (HF LlamaDecoderLayer as called at llama_model_utils.py:193-201,253-261,354-362,375-383)
+// With `sr` the M rows are sr->n_seqs sequences' (SeqRows), x_ld floats apart.
 // ---------------------------------------------------------------------------------------------
-static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base_len, int pos_off) {
+static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base_len, int pos_off,
+                         const SeqRows* sr = nullptr) {
   const lsk_config& c = e->cfg;
   LayerWeights& L = e->layers[li];
   float* x = e->hidden + (size_t)row0 * c.hidden;
+  const int x_ld = sr ? sr->x_ld : c.hidden;
   __nv_bfloat16* kp = e->kpool + (size_t)li * e->pool_layer_elems;
   __nv_bfloat16* vp = e->vpool + (size_t)li * e->pool_layer_elems;
   const bool tp = c.tp_size > 1;
@@ -622,12 +644,17 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
     GemmArgs a{};
     a.W = reinterpret_cast<const uint4*>(L.wqkv);
     a.M = M;
-    a.x_f32 = x; a.x_ld = c.hidden; a.norm_w = L.ln1; a.eps = c.rms_eps;
+    a.x_f32 = x; a.x_ld = x_ld; a.norm_w = L.ln1; a.eps = c.rms_eps;
     a.q_out = e->qbuf; a.q_ld = e->q_rows;
     a.kpool = kp; a.vpool = vp; a.page_table = e->page_table;
     a.base_len = base_len; a.pos_off = pos_off; a.rope = e->rope; a.head_dim = c.head_dim;
     a.q_rows = e->q_rows; a.kv_rows = e->kv_rows; a.n_kv_heads = e->kv_heads_l;
-    TRY((launch_gemm<PRO_RMS, EPI_QKV>(e, e->p_qkv, a)));
+    if (sr) {
+      a.seq_rows = sr->seq_rows; a.len_stride = sr->len_stride; a.seq_pages = sr->seq_pages;
+      TRY((launch_gemm<PRO_RMS, EPI_QKV_SEQS>(e, e->p_qkv, a)));
+    } else {
+      TRY((launch_gemm<PRO_RMS, EPI_QKV>(e, e->p_qkv, a)));
+    }
   }
   if (!(e->ablate & (1u << CLS_ATTN))) {  // attention over the paged cache
     e->cur_class = CLS_ATTN;
@@ -637,7 +664,13 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
     a.base_len = base_len; a.pos_off = pos_off; a.M = M; a.group = e->group;
     a.n_kv_heads = e->kv_heads_l; a.n_splits = e->n_splits;
     a.scale = 1.0f / sqrtf((float)c.head_dim);
-    TRY(launch_attention(e, a, c.head_dim));
+    if (sr) {   // one piece per sequence (attn_piece_kernel's sequence grid)
+      a.M = sr->seq_rows;
+      const AttnPieces pz{nullptr, (e->group * M + 15) / 16 * 16, sr->seq_rows, sr->len_stride, sr->seq_pages};
+      TRY(launch_attention(e, a, c.head_dim, &pz, sr->n_seqs));
+    } else {
+      TRY(launch_attention(e, a, c.head_dim));
+    }
   }
   if (!(e->ablate & (1u << CLS_O))) {  // O projection (+ residual, or all-reduce then residual under TP)
     e->cur_class = CLS_O;
@@ -646,7 +679,7 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
     a.M = M;
     a.x_bf16 = e->attn_out; a.xb_ld = e->q_rows;
     if (!tp) {
-      a.out_f32 = x; a.out_ld = c.hidden;
+      a.out_f32 = x; a.out_ld = x_ld;
       TRY((launch_gemm<PRO_BF16, EPI_RESID>(e, e->p_o, a)));
     } else if (e->peer_ok && e->peer_mode == 2) {
       TRY(emit_gemm_push_resid(e, e->p_o, a, x));
@@ -661,7 +694,7 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
     GemmArgs a{};
     a.W = reinterpret_cast<const uint4*>(L.wgu);
     a.M = M;
-    a.x_f32 = x; a.x_ld = c.hidden; a.norm_w = L.ln2; a.eps = c.rms_eps;
+    a.x_f32 = x; a.x_ld = x_ld; a.norm_w = L.ln2; a.eps = c.rms_eps;
     a.act = e->act; a.act_ld = e->inter_l_pad;
     TRY((launch_gemm<PRO_RMS, EPI_SILU>(e, e->p_gu, a)));
   }
@@ -672,7 +705,7 @@ static int enqueue_layer(lsk_engine* e, int li, int row0, int M, const int* base
     a.M = M;
     a.x_bf16 = e->act; a.xb_ld = e->inter_l_pad;
     if (!tp) {
-      a.out_f32 = x; a.out_ld = c.hidden;
+      a.out_f32 = x; a.out_ld = x_ld;
       TRY((launch_gemm<PRO_BF16, EPI_RESID>(e, e->p_d, a)));
     } else if (e->peer_ok && e->peer_mode == 2) {
       TRY(emit_gemm_push_resid(e, e->p_d, a, x));
@@ -891,14 +924,14 @@ static int emit_ar_commit(lsk_engine* e) {
   return LSK_OK;
 }
 
-// Final RMSNorm + the mma.sync LM head on M fp32 residual rows at x (row stride hidden): arg-max
+// Final RMSNorm + the mma.sync LM head on M fp32 residual rows at x (row stride x_ld; 0: hidden): arg-max
 // candidates into cand_*, and the logits rows when `logits` is set.
-static int launch_lm_head_gemm(lsk_engine* e, const float* x, int M, float* logits) {
+static int launch_lm_head_gemm(lsk_engine* e, const float* x, int M, float* logits, int x_ld = 0) {
   const lsk_config& c = e->cfg;
   GemmArgs a{};
   a.W = reinterpret_cast<const uint4*>(e->lm_head);
   a.M = M;
-  a.x_f32 = x; a.x_ld = c.hidden;
+  a.x_f32 = x; a.x_ld = x_ld ? x_ld : c.hidden;
   a.norm_w = e->final_norm; a.eps = c.rms_eps;
   a.logits = logits; a.logits_ld = e->vocab_l_pad;
   a.n_valid_rows = e->vocab_l; a.vocab_off = e->vocab_off;
@@ -912,9 +945,10 @@ static int launch_lm_head_gemm(lsk_engine* e, const float* x, int M, float* logi
 // With no_repeat_ngram_size > 0 (NoRepeatNGramLogitsProcessor, generator_base.py:77-85) the logits
 // are materialised, the tokens that would repeat an n-gram of the sequence so far are set to -inf
 // (row r continues prompt ++ output ++ draft[0 .. j0 + r)), and the arg-max is taken from the
-// banned rows instead of the LM-head epilogue.
-static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0) {
+// banned rows instead of the LM-head epilogue.  x_ld: row stride of the M rows (0: hidden).
+static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0, int x_ld = 0) {
   const lsk_config& c = e->cfg;
+  if (!x_ld) x_ld = c.hidden;
   const bool ban = e->gen.no_repeat_ngram_size > 0;
   e->cur_class = CLS_LMHEAD;
   const float* x = e->hidden + (size_t)row0 * c.hidden;
@@ -923,13 +957,13 @@ static int enqueue_lm_head(lsk_engine* e, int row0, int M, int j0) {
     if (!(e->ablate & (1u << CLS_LMHEAD))) {
       LmHeadTcArgs t{};
       t.W = e->lm_head_tc; t.n_tiles = e->lm_tc_tiles; t.K = c.hidden; t.M = M; t.n_stages = e->lm_tc_stages;
-      t.x_f32 = x; t.x_ld = c.hidden; t.norm_w = e->final_norm; t.eps = c.rms_eps;
+      t.x_f32 = x; t.x_ld = x_ld; t.norm_w = e->final_norm; t.eps = c.rms_eps;
       t.logits = logits; t.logits_ld = e->vocab_l_pad; t.n_valid_rows = e->vocab_l; t.vocab_off = e->vocab_off;
       t.part_val = e->cand_val; t.part_idx = e->cand_idx;
       CU(launch(e, lmhead_tc_kernel, dim3(e->lm_tc_grid), dim3(kTcThreads),
                 lmhead_tc_smem_bytes(c.hidden, e->lm_tc_stages), t));
     }
-  } else if (!(e->ablate & (1u << CLS_LMHEAD))) TRY(launch_lm_head_gemm(e, x, M, logits));
+  } else if (!(e->ablate & (1u << CLS_LMHEAD))) TRY(launch_lm_head_gemm(e, x, M, logits, x_ld));
   e->cur_class = CLS_MISC;
   const float* cv = e->cand_val;
   const int* ci = e->cand_idx;
@@ -1110,6 +1144,41 @@ static int enqueue_round_adaptive(lsk_engine* e, int E, int d) {
   return enqueue_verify(e, E, d, &e->state->d_stop);
 }
 
+// Batched round (lsk_round_batch): the rows of enqueue_round(E, d) for each of B sequences, every
+// weight pass shared.  Sequence s owns hidden rows s * (d + 1) .. s * (d + 1) + d; draft step i runs
+// row i of every sequence (B rows, (d + 1) * hidden floats apart), the verify's layers >= E run all
+// B * (d + 1) rows, each sequence at its own positions, over its own KV slot (page-table view
+// page_table + s * P).  The GEMMs are batch-invariant and the attention partition is fixed by
+// absolute key index, so every row is computed as in a round of that sequence alone.
+static int enqueue_round_batch(lsk_engine* e, int E, int B, int d) {
+  const lsk_config& c = e->cfg;
+  const int* len = &e->bstate->len;
+  const int len_stride = (int)(sizeof(DevState) / sizeof(int));
+  const int P = e->n_pages / B;
+  const int stride = (d + 1) * c.hidden;
+  const SeqRows draft{B, 1, len_stride, P, stride};
+  const SeqRows verify{B, d + 1, len_stride, P, c.hidden};
+  const __nv_bfloat16* embed = e->embed;
+  e->cur_class = CLS_MISC;
+  CU(launch(e, embed_seq_tokens_kernel, dim3(B), dim3(256), 0, embed, c.hidden, (const DevState*)e->bstate,
+            e->hidden, stride));
+  for (int i = 0; i < d; ++i) {
+    for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, i, B, len, i, &draft));
+    TRY(enqueue_lm_head(e, i, B, i, stride));
+    e->cur_class = CLS_MISC;
+    CU(launch(e, finalize_embed_seqs_kernel, dim3(8, B), dim3(128), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e),
+              e->bstate, 1 + i, embed, c.hidden, e->hidden + (size_t)(i + 1) * c.hidden, stride));
+  }
+  for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, d, B, len, d, &draft));
+  for (int l = E; l < c.n_layers; ++l) TRY(enqueue_layer(e, l, 0, B * (d + 1), len, 0, &verify));
+  TRY(enqueue_lm_head(e, 0, B * (d + 1), 0));
+  e->cur_class = CLS_MISC;
+  CU(launch(e, accept_greedy_seqs_kernel, dim3(B), dim3(256), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e), d,
+            e->bstate, (const GenParams*)e->gen_dev, e->bres_dev, (const int*)e->batch_ctl,
+            (const int*)e->batch_ctl + kMaxRows));
+  return LSK_OK;
+}
+
 static int enqueue_ar(lsk_engine* e, int n_layers_run) {
   const lsk_config& c = e->cfg;
   const int* len = &e->state->len;
@@ -1263,6 +1332,9 @@ static MemTable mem_table(const lsk_config& c, const EngineShape& s, int sm_coun
   t.batch_buf = {8 * P * 4, S};
   t.view_table = {P * 4, S};
   t.piece_arrive = {(size_t)kPfTokens * s.kv_heads_l * 4, S};
+  t.batch_state = {(size_t)kMaxRows * sizeof(DevState), S};
+  t.batch_ctl = {(size_t)2 * kMaxRows * 4, S};
+  t.batch_arrive = {(size_t)kMaxRows * s.kv_heads_l * 4, S};
   t.peer_region = {peer_region_layout(c.tp_size, c.hidden).total, S};
   return t;
 }
@@ -1311,6 +1383,8 @@ static void plan_memory(const lsk_config& c, const EngineShape& s, const MemTabl
   if (packed)
     for (const MemBuf& b : {t.batch_buf, t.view_table, t.piece_arrive}) add(b, 1);
   if (u.tp_peer && c.tp_size > 1) add(t.peer_region, 1);
+  if (u.batch_seqs > 0)                                // sized for max_rows sequences, whatever the batch
+    for (const MemBuf& b : {t.batch_state, t.batch_ctl, t.batch_arrive}) add(b, 1);
 }
 
 static lsk_memory_plan plan_of(const int64_t* cat) {
@@ -1430,6 +1504,8 @@ int lsk_plan_memory(const lsk_config* cfg, int32_t sm_count, const lsk_memory_us
   if (uses->score_exits < 0 || uses->score_exits > LSK_MAX_EXITS || uses->accept_exits < 0 ||
       uses->accept_exits > LSK_MAX_EXITS)
     return fail(LSK_ERR_INVALID, "score_exits and accept_exits must be in [0, %d]", LSK_MAX_EXITS);
+  if (uses->batch_seqs < 0 || uses->batch_seqs > kMaxRows)
+    return fail(LSK_ERR_INVALID, "batch_seqs must be in [0, %d]", kMaxRows);
   const EngineShape s = engine_shape(*cfg, sm_count, !(cfg->flags & LSK_FLAG_NO_PREFILL_TC), uses->lm_head_tc != 0);
   int64_t cat[MEM_CATS] = {};
   plan_memory(*cfg, s, mem_table(*cfg, s, sm_count), *uses, cat);
@@ -1840,6 +1916,7 @@ int lsk_begin(lsk_engine* e, const lsk_generation* gen) {
   CU(cudaStreamSynchronize(e->stream));
   e->began = true;
   e->prefilled = false;
+  e->batch_n = 0;
   e->host_len = 0;
   return LSK_OK;
 }
@@ -1864,11 +1941,11 @@ int lsk_prefill(lsk_engine* e, const int32_t* ids, int32_t n) {
   TRY(peer_check(e));
   e->host_len = n - 1;
   e->prefilled = true;
+  e->batch_n = 0;
   return LSK_OK;
 }
 
-static void copy_result(const lsk_engine* e, lsk_round_out* out) {
-  const RoundResult& r = *e->res_host;
+static void copy_result(const RoundResult& r, lsk_round_out* out) {
   out->n_drafted = r.n_drafted;
   out->n_matches = r.n_matches;
   out->n_emitted = r.n_emitted;
@@ -1891,7 +1968,7 @@ int lsk_round(lsk_engine* e, int32_t d_req, lsk_round_out* out) {
                         ((long long)e->gen.no_repeat_ngram_size << 32);
   TRY(run_cached(e, key, [&]() { return enqueue_round(e, E, d_req); }));
   TRY(peer_check(e));
-  copy_result(e, out);
+  copy_result(*e->res_host, out);
   e->host_len = out->kv_len;
   return LSK_OK;
 }
@@ -1925,7 +2002,7 @@ int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_r
   e->adaptive = false;
   e->pdl_break = false;
   TRY(st);
-  copy_result(e, out);
+  copy_result(*e->res_host, out);
   if (draft_conf_out)
     for (int i = 0; i < out->n_drafted; ++i) draft_conf_out[i] = e->res_host->conf[i];
   e->host_len = out->kv_len;
@@ -1942,6 +2019,110 @@ int lsk_ar_step(lsk_engine* e, int32_t* token_out) {
   TRY(peer_check(e));
   *token_out = e->res_host->emitted_ids[0];
   e->host_len = e->res_host->kv_len;
+  return LSK_OK;
+}
+
+// What a batch of sequences needs of the generation lsk_begin set up: greedy, no n-gram ban, one GPU,
+// a self-speculation exit layer.
+static int check_batch_generation(const lsk_engine* e) {
+  if (e->gen.sample) return fail(LSK_ERR_INVALID, "batched generation is greedy only: sampling is not supported");
+  if (e->gen.no_repeat_ngram_size > 0)
+    return fail(LSK_ERR_INVALID, "batched generation does not support the n-gram ban (no_repeat_ngram_size %d)",
+                e->gen.no_repeat_ngram_size);
+  if (e->cfg.tp_size > 1) return fail(LSK_ERR_INVALID, "batched generation needs tp_size 1 (got %d)", e->cfg.tp_size);
+  const int E = e->gen.exit_layer;
+  if (E < 1 || E > e->cfg.n_layers)
+    return fail(LSK_ERR_INVALID, "self-speculation needs 1 <= exit_layer <= n_layers (got %d)", E);
+  return LSK_OK;
+}
+
+// Sequence s of a batch of n sequences owns logical pages [s * P, (s + 1) * P) of the pool, P = n_pages / n:
+// its position p is logical position s * 64 * P + p.
+static int batch_slot_positions(const lsk_engine* e, int n) { return e->n_pages / n * kPageTokens; }
+
+int lsk_prefill_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
+                      int32_t* slot_positions_out) {
+  if (!e || !ids || !offsets) return fail(LSK_ERR_INVALID, "null argument");
+  if (!e->began) return fail(LSK_ERR_STATE, "lsk_begin must precede lsk_prefill_batch");
+  TRY(check_batch_generation(e));
+  if (n_seqs < 1 || n_seqs > e->max_rows)
+    return fail(LSK_ERR_INVALID, "n_seqs %d outside [1, %d]", n_seqs, e->max_rows);
+  if (offsets[0] != 0) return fail(LSK_ERR_INVALID, "offsets[0] must be 0 (got %d)", offsets[0]);
+  const int slot = batch_slot_positions(e, n_seqs);
+  for (int j = 0; j < n_seqs; ++j) {
+    const int n = offsets[j + 1] - offsets[j];
+    if (n < 1) return fail(LSK_ERR_INVALID, "prompt %d is empty (offsets %d, %d)", j, offsets[j], offsets[j + 1]);
+    for (int i = offsets[j]; i < offsets[j + 1]; ++i)
+      if (ids[i] < 0 || ids[i] >= e->cfg.vocab) return fail(LSK_ERR_INVALID, "prompt %d: token id %d out of range", j, ids[i]);
+    if (n + 1 > slot)
+      return fail(LSK_ERR_CTX, "prompt %d of %d tokens does not fit its slot of %d positions (%d sequences)", j, n, slot,
+                  n_seqs);
+  }
+  const MemTable& t = e->sizes;
+  TRY(alloc_once(e, &e->bstate, t.batch_state));
+  TRY(alloc_once(e, &e->batch_ctl, t.batch_ctl));
+  TRY(alloc_once(e, &e->batch_arrive, t.batch_arrive, true));
+  if (!e->bres_host) {
+    CU(cudaHostAlloc((void**)&e->bres_host, kMaxRows * sizeof(RoundResult), cudaHostAllocMapped));
+    memset(e->bres_host, 0, kMaxRows * sizeof(RoundResult));
+    CU(cudaHostGetDevicePointer((void**)&e->bres_dev, e->bres_host, 0));
+  }
+  e->prefilled = false;
+  e->batch_n = 0;
+  e->host_len = 0;
+  CU(cudaEventRecord(e->ev0, e->stream));
+  CU(cudaMemsetAsync(e->bstate, 0, t.batch_state.bytes, e->stream));
+  // prompt j through lsk_prefill's route, over its slot's page-table view
+  int* const table = e->page_table;
+  for (int j = 0; j < n_seqs; ++j) {
+    const int32_t* p = ids + offsets[j];
+    const int n = offsets[j + 1] - offsets[j];
+    CU(cudaMemcpyAsync(e->d_prompt, p, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+    e->page_table = table + (size_t)j * (slot / kPageTokens);
+    const int st = enqueue_prompt_rows(e, n - 1, e->cfg.n_layers, nullptr, 0, {});
+    e->page_table = table;
+    TRY(st);
+    set_state_kernel<<<1, 1, 0, e->stream>>>(e->bstate + j, n - 1, p[n - 1], 0, n);
+    CU(cudaGetLastError());
+  }
+  CU(cudaEventRecord(e->ev1, e->stream));
+  CU(cudaEventSynchronize(e->ev1));
+  CU(cudaEventElapsedTime(&e->last_ms, e->ev0, e->ev1));
+  e->batch_len.assign(n_seqs, 0);
+  for (int j = 0; j < n_seqs; ++j) e->batch_len[j] = offsets[j + 1] - offsets[j] - 1;
+  e->batch_n = n_seqs;
+  if (slot_positions_out) *slot_positions_out = slot;
+  return LSK_OK;
+}
+
+int lsk_round_batch(lsk_engine* e, int32_t d_req, const int32_t* d_seq, const int32_t* active,
+                    lsk_round_out* outs) {
+  if (!e || !outs) return fail(LSK_ERR_INVALID, "null argument");
+  if (!e->batch_n) return fail(LSK_ERR_STATE, "lsk_prefill_batch must precede lsk_round_batch");
+  TRY(check_batch_generation(e));
+  const int B = e->batch_n, E = e->gen.exit_layer;
+  if (d_req < 0 || B * (d_req + 1) > e->max_rows)
+    return fail(LSK_ERR_INVALID, "%d sequences x (d_req %d + 1) rows exceed the %d rows of a step", B, d_req,
+                e->max_rows);
+  int ctl[2 * kMaxRows] = {};
+  for (int s = 0; s < B; ++s) {
+    ctl[s] = d_seq ? d_seq[s] : d_req;
+    ctl[kMaxRows + s] = active ? (active[s] != 0) : 1;
+    if (ctl[s] < 0 || ctl[s] > d_req)
+      return fail(LSK_ERR_INVALID, "d_seq[%d] = %d outside [0, d_req %d]", s, ctl[s], d_req);
+  }
+  const int slot = batch_slot_positions(e, B);
+  for (int s = 0; s < B; ++s)
+    if (e->batch_len[s] + d_req + 2 > slot)
+      return fail(LSK_ERR_CTX, "sequence %d: context %d + %d exceeds its slot of %d positions", s, e->batch_len[s],
+                  d_req + 1, slot);
+  CU(cudaMemcpyAsync(e->batch_ctl, ctl, sizeof(ctl), cudaMemcpyHostToDevice, e->stream));
+  const long long key = ((long long)E << 20) | ((long long)d_req << 8) | 16 | 1 | ((long long)B << 40);
+  TRY(run_cached(e, key, [&]() { return enqueue_round_batch(e, E, B, d_req); }));
+  for (int s = 0; s < B; ++s) {
+    copy_result(e->bres_host[s], &outs[s]);
+    e->batch_len[s] = outs[s].kv_len;
+  }
   return LSK_OK;
 }
 
@@ -1973,7 +2154,7 @@ int lsk_profile_round(lsk_engine* e, int32_t d_req, lsk_round_out* out, float* c
     cudaEventDestroy(pe.second.second);
   }
   e->prof_events.clear();
-  copy_result(e, out);
+  copy_result(*e->res_host, out);
   e->host_len = out->kv_len;
   return LSK_OK;
 }
@@ -2071,6 +2252,7 @@ static int score_sequence(lsk_engine* e, const int32_t* ids, int n, const int32_
   const WarpParams wp = accept_out ? WarpParams{sampling->temperature, sampling->top_k, sampling->top_p}
                                    : WarpParams{1.f, 0, 1.f};
   e->prefilled = false;
+  e->batch_n = 0;
   e->host_len = 0;
   auto head = [&](int j, const float* x, int r0, int rc, int M) -> int {
     TRY(enqueue_score_head(e, x, M, e->d_prompt + r0 + 1, r0, e->score_lp + j * P, e->score_greedy + j * P));
@@ -2184,6 +2366,7 @@ static int score_packed(lsk_engine* e, int E, const std::vector<ScorePrefix>& pr
   TRY(alloc_scoring(e, 1, true));
   const int m_attn = prompt_attn_rows(e->cfg.head_dim, e->group);
   e->prefilled = false;
+  e->batch_n = 0;
   e->host_len = 0;
 
   struct Member { const ScorePrefix* p; int b0, b1; };   // a prefix with its branches [b0, b1) in the group

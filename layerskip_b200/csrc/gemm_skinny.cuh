@@ -28,7 +28,9 @@ namespace lsk {
 enum { PRO_RMS = 0, PRO_BF16 = 1 };
 // EPI_PUSH (tensor parallel, opt-in): like EPI_STORE, but the fp32 tile goes straight into every
 // rank's peer-visible region over NVLink while the kernel is still streaming (tp_peer.cuh)
-enum { EPI_QKV = 0, EPI_RESID = 1, EPI_STORE = 2, EPI_SILU = 3, EPI_LMHEAD = 4, EPI_PUSH = 5 };
+// EPI_QKV_SEQS (batched rounds): EPI_QKV on the rows of several sequences (GemmArgs::seq_rows); a
+// separate instantiation, so the single-sequence epilogue stays as it is
+enum { EPI_QKV = 0, EPI_RESID = 1, EPI_STORE = 2, EPI_SILU = 3, EPI_LMHEAD = 4, EPI_PUSH = 5, EPI_QKV_SEQS = 6 };
 
 constexpr int kGemmWarps = 16;                       // consumer warps (LDS + MMA)
 constexpr int kEpiWarps = 3;                         // reduction / epilogue warps
@@ -87,6 +89,10 @@ struct GemmArgs {
   const int* page_table;
   const int* base_len;
   int pos_off;
+  // EPI_QKV_SEQS: row m belongs to sequence s = m / seq_rows, sits at position
+  // base_len[s * len_stride] + pos_off + m % seq_rows and writes through the page-table view
+  // page_table + s * seq_pages (EPI_QKV: every row is one sequence's, at *base_len + pos_off + m)
+  int seq_rows, len_stride, seq_pages;
   const float2* rope;    // [max_pos][head_dim / 2] (cos, sin)
   int head_dim;
   int q_rows;            // local q rows (heads * head_dim)
@@ -100,6 +106,14 @@ struct GemmArgs {
   float* part_val;       // [grid][16]
   int* part_idx;
 };
+
+// EPI_QKV_SEQS: position of token row m, and the first page-table entry of its sequence's view in
+// *view
+__device__ __forceinline__ int qkv_seq_pos(const GemmArgs& a, int m, int* view) {
+  const int s = m / a.seq_rows;
+  *view = s * a.seq_pages;
+  return a.base_len[s * a.len_stride] + a.pos_off + (m - s * a.seq_rows);
+}
 
 __host__ __device__ inline int gemm_x_stride_bytes(int kcols) {
   return ((2 * kcols + 127) / 128) * 128 + 64;   // == 64 (mod 128): conflict-free LDS.128
@@ -501,11 +515,12 @@ __device__ __forceinline__ void gemm_epilogue_role(const GemmArgs& a, const Gemm
     }
     // EPI_QKV: RoPE factors and KV page of this thread's items, fetched BEFORE the tile arrives
     // (the committed length is constant while the kernel runs) — same idea as old_resid
+    constexpr bool kSeqs = EPI == EPI_QKV_SEQS;
     constexpr int kQkvItems = (kMaxTilesPerPass * NT * 64 + kEpiThreads - 1) / kEpiThreads;
     float2 q_cs[kQkvItems];
     int q_page[kQkvItems];
-    if (EPI == EPI_QKV) {
-      const int base_pos = *a.base_len + a.pos_off;
+    if (EPI == EPI_QKV || kSeqs) {
+      const int base_pos = kSeqs ? 0 : *a.base_len + a.pos_off;
       const int half = a.head_dim >> 1;
 #pragma unroll
       for (int k = 0; k < kQkvItems; ++k) {
@@ -516,12 +531,14 @@ __device__ __forceinline__ void gemm_epilogue_role(const GemmArgs& a, const Gemm
           const int tok = itx & 7, r = (itx >> 3) & 7, n = (itx >> 6) % NT, j = (itx >> 6) / NT;
           const int m = n * 8 + tok, tile = slot * TPP + j;
           if (m < a.M && tile < a.n_tiles) {
-            const int pr = tile * 16, pos = base_pos + m;
+            const int pr = tile * 16;
+            int pos = base_pos + m, view = 0;
+            if (kSeqs) pos = qkv_seq_pos(a, m, &view);
             if (pr < a.q_rows + a.kv_rows) {
               const int rel = pr < a.q_rows ? pr : pr - a.q_rows;
               q_cs[k] = a.rope[(size_t)pos * half + ((rel % a.head_dim) >> 4) * 8 + r];
             }
-            if (pr >= a.q_rows) q_page[k] = a.page_table[pos >> 6];
+            if (pr >= a.q_rows) q_page[k] = a.page_table[view + (pos >> 6)];
           }
         }
       }
@@ -536,7 +553,7 @@ __device__ __forceinline__ void gemm_epilogue_role(const GemmArgs& a, const Gemm
       return s;
     };
 
-    if (EPI == EPI_QKV || EPI == EPI_SILU) {
+    if (EPI == EPI_QKV || kSeqs || EPI == EPI_SILU) {
       const int items = TPP * NT * 64;
 #pragma unroll
       for (int kq = 0; kq < kQkvItems; ++kq) {
@@ -552,7 +569,8 @@ __device__ __forceinline__ void gemm_epilogue_role(const GemmArgs& a, const Gemm
           a.act[(size_t)m * a.act_ld + tile * 8 + r] = __float2bfloat16_rn(sg * hi);
         } else {
           const int pr = tile * 16;                     // first packed row of the tile
-          const int pos = *a.base_len + a.pos_off + m;
+          int view;
+          const int pos = kSeqs ? qkv_seq_pos(a, m, &view) : *a.base_len + a.pos_off + m;
           const int HD = a.head_dim, half = HD >> 1;
           if (pr < a.q_rows + a.kv_rows) {              // q or k: rotary pair (d, d + HD/2)
             const bool is_q = pr < a.q_rows;

@@ -146,6 +146,47 @@ __global__ void finalize_embed_kernel(const float* __restrict__ cand_val,
   }
 }
 
+// Batched rounds: sequence s's rows are row_ld floats apart.  embed_seq_tokens_kernel embeds
+// st[s].tok[0] into rows + s * row_ld (grid n_seqs); finalize_embed_seqs_kernel is
+// finalize_embed_kernel for candidate row s = blockIdx.y: its token goes to st[s].tok[slot] and is
+// embedded into rows + s * row_ld (grid (slices, n_seqs)).
+__global__ void embed_seq_tokens_kernel(const __nv_bfloat16* __restrict__ embed, int hidden,
+                                        const DevState* __restrict__ st, float* __restrict__ rows,
+                                        int row_ld) {
+  pdl_launch_dependents();
+  pdl_wait();
+  embed_row(embed, hidden, st[blockIdx.x].tok[0], rows + (size_t)blockIdx.x * row_ld, threadIdx.x,
+            blockDim.x);
+}
+
+__global__ void finalize_embed_seqs_kernel(const float* __restrict__ cand_val,
+                                           const int* __restrict__ cand_idx, int n_cand,
+                                           DevState* __restrict__ st, int slot,
+                                           const __nv_bfloat16* __restrict__ embed, int hidden,
+                                           float* __restrict__ rows, int row_ld) {
+  __shared__ int s_tok;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int s = blockIdx.y;
+  if (threadIdx.x < 32) {
+    const int tok = reduce_candidates(cand_val, cand_idx, n_cand, s, threadIdx.x);
+    if (threadIdx.x == 0) {
+      s_tok = tok;
+      if (blockIdx.x == 0) st[s].tok[slot] = tok;
+    }
+  }
+  __syncthreads();
+  const int per = (hidden / 4 + gridDim.x - 1) / gridDim.x;   // float4 per CTA
+  const int lo = blockIdx.x * per, hi = min(hidden / 4, lo + per);
+  const uint2* src = reinterpret_cast<const uint2*>(embed + (size_t)s_tok * hidden);
+  float* dst_row = rows + (size_t)s * row_ld;
+  for (int i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+    const uint2 v = src[i];
+    *reinterpret_cast<float4*>(dst_row + i * 4) =
+        make_float4(bf16_lo(v.x), bf16_hi(v.x), bf16_lo(v.y), bf16_hi(v.y));
+  }
+}
+
 // Per-generation constants on the device.
 struct GenParams {
   int n_eos;
@@ -229,6 +270,37 @@ __global__ void accept_greedy_kernel(const float* __restrict__ cand_val,
   }
   __syncthreads();
   if (threadIdx.x == 0) accept_commit(s_ver, d, st, *gp, res, seq, hist, d_stop);
+}
+
+// Batched round: one CTA per sequence s = blockIdx.x, whose verify rows are candidate rows
+// s * (d + 1) .. s * (d + 1) + d.  An active sequence accepts and commits as a round of d_seq[s]
+// drafts would (accept_commit with d_seq[s] as d_stop: its rows past d_seq[s] are causally invisible
+// to the kept ones) into st[s] and res[s]; an inactive one commits nothing and reports no tokens.
+__global__ void accept_greedy_seqs_kernel(const float* __restrict__ cand_val,
+                                          const int* __restrict__ cand_idx, int n_cand, int d,
+                                          DevState* __restrict__ st, const GenParams* __restrict__ gp,
+                                          RoundResult* __restrict__ res, const int* __restrict__ d_seq,
+                                          const int* __restrict__ active) {
+  __shared__ int s_ver[kMaxRows];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int s = blockIdx.x;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int row = warp; row <= d; row += blockDim.x >> 5) {
+    const int tok = reduce_candidates(cand_val, cand_idx, n_cand, s * (d + 1) + row, lane);
+    if (lane == 0) s_ver[row] = tok;
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  if (active[s]) {
+    accept_commit(s_ver, d, &st[s], *gp, &res[s], 0, nullptr, &d_seq[s]);
+    return;
+  }
+  RoundResult* r = &res[s];
+  r->n_drafted = r->n_matches = r->n_emitted = 0;
+  r->kv_len = st[s].len;
+  __threadfence_system();
+  *reinterpret_cast<volatile int*>(&r->seq) = 0;
 }
 
 // Autoregressive commit (autoregressive_generator.py:62-76): token = argmax(row 0).

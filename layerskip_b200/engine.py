@@ -17,6 +17,15 @@ from . import _lib
 from .weights import LlamaArch, SyntheticLlama, iter_state_dict
 
 
+def batch_slot_positions(max_ctx: int, n_seqs: int) -> int:
+    """Positions each sequence of an `n_seqs` batch owns in an engine built with `max_ctx`: the pool's
+    ceil(max_ctx / 64) pages split into n_seqs slots of whole 64-token pages (engine.cu:
+    batch_slot_positions)."""
+    if n_seqs < 1:
+        raise ValueError(f"n_seqs must be >= 1 (got {n_seqs})")
+    return ((max_ctx + 63) // 64) // n_seqs * 64
+
+
 @dataclass
 class RoundOutput:
     """One speculation round as seen by the host (lsk_round_out)."""
@@ -80,6 +89,7 @@ class Engine:
             _lib.check(self._lib.lsk_create(C.byref(cfg), C.byref(handle)))
         self._h = handle
         self._exit_layer = -1
+        self._batch_n = 0                  # sequences of the last prefill_batch
         # token rows one step can carry (engine.cu: max_rows): 16 when the host planner finds a
         # schedule for the 16-row RMSNorm GEMM at K = hidden (whole rows resident up to hidden 4096,
         # K-chunked normalisation above), else 8
@@ -192,6 +202,50 @@ class Engine:
             draft=list(out.draft_ids[:out.n_drafted]),
             verified=list(out.verified_ids[:out.n_drafted + 1]), kv_len=out.kv_len,
             draft_confidence=[float(x) for x in conf[:out.n_drafted]])
+
+    @staticmethod
+    def _round_output(out) -> RoundOutput:
+        return RoundOutput(
+            n_drafted=out.n_drafted, n_matches=out.n_matches,
+            emitted=list(out.emitted_ids[:out.n_emitted]),
+            draft=list(out.draft_ids[:out.n_drafted]),
+            verified=list(out.verified_ids[:out.n_drafted + 1]) if out.n_emitted else [],
+            kv_len=out.kv_len)
+
+    # ------------------------------------------------------------------ batched generation
+    def prefill_batch(self, prompts: Sequence[Sequence[int]]) -> int:
+        """Prefill every prompt into its own slot of the KV pool (after `begin`, greedy, no n-gram ban,
+        one GPU).  Returns the positions each slot holds: `batch_slot_positions(max_ctx, len(prompts))`.
+        Each prompt is prefilled exactly as `prefill` would prefill it alone."""
+        prompts = [[int(t) for t in p] for p in prompts]
+        offsets = [0]
+        for p in prompts:
+            offsets.append(offsets[-1] + len(p))
+        flat = [t for p in prompts for t in p]
+        arr = (C.c_int32 * max(len(flat), 1))(*flat)
+        off = (C.c_int32 * len(offsets))(*offsets)
+        slot = C.c_int32()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_prefill_batch(self._h, arr, off, len(prompts), C.byref(slot)))
+        self._batch_n = len(prompts)
+        return slot.value
+
+    def round_batch(self, d_req: int, d_seq: Optional[Sequence[int]] = None,
+                    active: Optional[Sequence[bool]] = None) -> List[RoundOutput]:
+        """One round for every sequence of the batch (len(prompts) * (d_req + 1) <= max_rows): sequence s
+        drafts d_seq[s] <= d_req tokens (default d_req) and, when active (default), commits exactly what
+        `round(d_seq[s])` of that sequence alone would.  An inactive sequence commits nothing and gets
+        an empty RoundOutput (no tokens, kv_len unchanged)."""
+        n = self._batch_n
+        for name, v in (("d_seq", d_seq), ("active", active)):
+            if v is not None and len(v) != n:
+                raise ValueError(f"{name} has {len(v)} entries for a batch of {n} sequences")
+        ds = (C.c_int32 * n)(*[int(x) for x in d_seq]) if d_seq is not None else None
+        act = (C.c_int32 * n)(*[int(bool(x)) for x in active]) if active is not None else None
+        outs = (_lib.lsk_round_out * (_lib.LSK_MAX_SPEC + 1))()    # up to max_rows sequences
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_round_batch(self._h, int(d_req), ds, act, outs))
+        return [self._round_output(o) for o in outs[:n]]
 
     KERNEL_CLASSES = ("qkv", "attention", "o_proj", "gate_up", "down", "lm_head", "small", "comm")
 

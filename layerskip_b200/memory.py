@@ -20,14 +20,15 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
                 keep_logits: bool = False, lm_head_tc: bool = False, prefill_tc: bool = True,
                 scoring: bool = False, batch_scoring: bool = False, score_exits: int = 0,
                 score_exits_sampled: bool = False, adaptive: bool = False, ngram_ban: bool = False,
-                sm_count: int = 132) -> Dict[str, int]:
+                batch_seqs: int = 0, sm_count: int = 132) -> Dict[str, int]:
     """Bytes the engine allocates on ONE rank of a GPU with `sm_count` SMs (132: H100 SXM).  Keys:
     weights, embed, lm_head, kv_pool, scratch, total (+ weights_source_peak: the largest single
     tensor staged on the GPU while loading).
     Beyond what `lsk_create` allocates, each flag adds what its first call allocates: `sampling` and
     `ngram_ban` a `begin` with sampling / the n-gram ban, `adaptive` a `round_adaptive`, `scoring`
     an `lsk_score`, `score_exits` = k an `lsk_score_exits` with k exits (`score_exits_sampled`: with
-    acceptance probabilities), `batch_scoring` an `lsk_score_batch` or `lsk_score_prefixed`.  With
+    acceptance probabilities), `batch_scoring` an `lsk_score_batch` or `lsk_score_prefixed`,
+    `batch_seqs` > 0 an `lsk_prefill_batch` of up to that many sequences (the same buffers for any count).  With
     tp_size > 1 the peer region of the one-shot collectives is counted."""
     cfg = arch.lsk_config(max_ctx, tp_size=tp_size,
                           flags=(_lib.LSK_FLAG_KEEP_LOGITS if keep_logits else 0) |
@@ -35,7 +36,8 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
     uses = _lib.lsk_memory_uses(lm_head_tc=int(lm_head_tc), sampling=int(sampling), ngram_ban=int(ngram_ban),
                                 adaptive=int(adaptive), score_exits=max(score_exits, int(scoring)),
                                 accept_exits=score_exits if score_exits_sampled else 0,
-                                packed_scoring=int(batch_scoring), tp_peer=int(tp_size > 1))
+                                packed_scoring=int(batch_scoring), tp_peer=int(tp_size > 1),
+                                batch_seqs=int(batch_seqs))
     plan = _lib.lsk_memory_plan()
     _lib.check(_lib.load().lsk_plan_memory(C.byref(cfg), sm_count, C.byref(uses), C.byref(plan)))
     out = {name: getattr(plan, name) for name, _ in _lib.lsk_memory_plan._fields_}

@@ -16,7 +16,7 @@ from typing import Any, Dict, List, Optional, Tuple
 
 import torch
 
-from .engine import Engine
+from .engine import Engine, batch_slot_positions
 from .plugin import GenerationConfig, GenerationStrategy, GenerationStrategyResult
 from .weights import LlamaArch, SyntheticLlama
 
@@ -174,6 +174,69 @@ class B200SelfSpeculativeGenerationStrategy(GenerationStrategy):
                     break
         return GenerationStrategyResult(predicted_tokens=output_ids,
                                         acceptance_rate=matches / drafted)   # :96-99
+
+    def generate_batch(self, model, prompts: List[List[int]], eos_token_ids: List[int],
+                       generation_config: GenerationConfig, logits_processors=None, stopping_criteria=None,
+                       streamer=None) -> List[GenerationStrategyResult]:
+        """Greedy self-speculative generation of several prompts at once: every round runs all the
+        sequences still generating through the same weight passes (`Engine.round_batch`).  Result j
+        equals `generate_token_ids(model, prompts[j], ...)` with the same config: the outer loop
+        below is the reference's, per sequence (max_steps clamp, acceptance accounting, EOS
+        truncation), and each sequence's rounds are bit-identical to its rounds alone.  Sampling,
+        logits processors, stopping criteria and streamers are not supported here.  The prompts share
+        the KV pool: each gets ceil(max_ctx / 64) // len(prompts) whole 64-token pages."""
+        cfg = generation_config
+        if cfg.sample:
+            raise NotImplementedError("generate_batch is greedy only: set sample=False")
+        if logits_processors or cfg.no_repeat_ngram_size:
+            raise NotImplementedError("generate_batch supports no logits processors (no n-gram ban)")
+        if stopping_criteria or cfg.stop_words:
+            raise NotImplementedError("generate_batch supports no stopping criteria (stop_words); use eos ids")
+        if streamer is not None:
+            raise NotImplementedError("generate_batch does not stream")
+        if getattr(cfg, "draft_confidence_threshold", 0.0):
+            raise NotImplementedError("generate_batch does not support draft_confidence_threshold")
+        prompts = [[int(t) for t in p] for p in prompts]
+        if not prompts:
+            return []
+        if any(len(p) == 0 for p in prompts):
+            raise ValueError("every prompt needs at least one token")
+        eng = self.engines.get(model)
+        _check_num_speculations(cfg, eng)
+        n, D = len(prompts), cfg.num_speculations
+        if n * (D + 1) > eng.max_rows:
+            raise ValueError(f"{n} prompts x (num_speculations {D} + 1) rows exceed the {eng.max_rows} token rows "
+                             "of a step; generate fewer prompts at once or draft fewer tokens")
+        slot = batch_slot_positions(eng.max_ctx, n)
+        need = max(len(p) for p in prompts) + cfg.max_steps + D + 1
+        if need > slot:
+            raise ValueError(f"the longest prompt + max_steps ({cfg.max_steps}) + num_speculations ({D}) + 1 needs "
+                             f"{need} KV positions but each of {n} prompts gets {slot} (max_ctx={eng.max_ctx}); "
+                             "construct the strategy with a larger max_ctx or generate fewer prompts at once")
+        eng.begin(exit_layer=cfg.exit_layer, max_steps=cfg.max_steps, eos_token_ids=eos_token_ids, sample=False)
+        eng.prefill_batch(prompts)
+        outs: List[List[int]] = [[] for _ in prompts]
+        matches, drafted = [0] * n, [0] * n
+        active = [cfg.max_steps > 0] * n
+        while any(active):
+            d_seq = [min(D, cfg.max_steps - len(o) - 1) if a else 0 for o, a in zip(outs, active)]
+            d_req = max(d for d, a in zip(d_seq, active) if a)
+            rounds = eng.round_batch(d_req, d_seq, active)
+            for s, r in enumerate(rounds):
+                if not active[s]:
+                    continue
+                outs[s].extend(r.emitted)
+                matches[s] += r.n_matches
+                drafted[s] += r.n_drafted
+                for eos in eos_token_ids:
+                    if eos in outs[s]:
+                        outs[s] = outs[s][: outs[s].index(eos)]
+                        active[s] = False
+                        break
+                if len(outs[s]) >= cfg.max_steps:
+                    active[s] = False
+        return [GenerationStrategyResult(predicted_tokens=o, acceptance_rate=m / d if d else None)
+                for o, m, d in zip(outs, matches, drafted)]
 
 
 class B200AutoRegressiveGenerationStrategy(GenerationStrategy):
