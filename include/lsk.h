@@ -360,6 +360,17 @@ int lsk_test_gemm(const void* packed_dev, int64_t n, int64_t k, const void* x_bf
 int lsk_test_attn(const void* q_dev, const void* k_dev, const void* v_dev, int32_t n_heads,
                   int32_t n_kv_heads, int32_t head_dim, int32_t ctx, int32_t m, int32_t n_splits,
                   const int32_t* page_perm_host, void* out_dev, int32_t iters, float* avg_ms_out);
+/* The same attention over several sequences in one launch, as a batched round (lsk_round_batch)
+ * launches it: sequence s has seq_rows query rows (q / out rows s * seq_rows ..) at positions
+ * ctx_host[s] - seq_rows .. ctx_host[s] - 1, and its keys k / v natural
+ * [n_seqs][n_kv_heads][slot_positions][head_dim] bf16 fill logical pages [s * P, (s + 1) * P) of one
+ * pool, P = slot_positions / 64; page_perm_host (nullable) permutes all n_seqs * P pages.  Refuses
+ * n_seqs * seq_rows > 16, ctx_host[s] outside [seq_rows, slot_positions], a slot that is not a
+ * multiple of 64 and n_splits outside [1, 8]. */
+int lsk_test_attn_seqs(const void* q_dev, const void* k_dev, const void* v_dev, int32_t n_heads,
+                       int32_t n_kv_heads, int32_t head_dim, int32_t n_seqs, int32_t seq_rows,
+                       const int32_t* ctx_host, int32_t slot_positions, int32_t n_splits,
+                       const int32_t* page_perm_host, void* out_dev);
 /* wgmma LM head (csrc/lmhead_tc.cuh, opt-in): logits[m, n] = rmsnorm(x)[m, :] . W[n, :] with
  * W natural bf16 [n, k], x fp32 [m, k], norm_w bf16 [k]; writes fp32 logits [m, n] and per row the
  * arg-max (lowest index wins).  All pointers are device pointers. */

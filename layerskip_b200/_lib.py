@@ -147,6 +147,9 @@ SIGNATURES = {
     "lsk_test_attn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                 C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_void_p,
                                 C.c_int32, C.POINTER(C.c_float)]),
+    "lsk_test_attn_seqs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                     C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int32,
+                                     C.POINTER(C.c_int32), C.c_void_p]),
     "lsk_test_lmhead_tc": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                      C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_int32, C.POINTER(C.c_float)]),

@@ -2057,6 +2057,9 @@ int lsk_prefill_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets,
     if (n + 1 > slot)
       return fail(LSK_ERR_CTX, "prompt %d of %d tokens does not fit its slot of %d positions (%d sequences)", j, n, slot,
                   n_seqs);
+    // the slot rounds max_ctx up to whole pages: a prompt lsk_prefill refuses has no solo run to match
+    if (n + 1 > e->cfg.max_ctx)
+      return fail(LSK_ERR_CTX, "prompt %d of %d tokens exceeds max_ctx %d", j, n, e->cfg.max_ctx);
   }
   const MemTable& t = e->sizes;
   TRY(alloc_once(e, &e->bstate, t.batch_state));
@@ -2929,6 +2932,72 @@ int lsk_test_attn(const void* q, const void* k, const void* v, int32_t n_heads, 
     CU(cudaEventElapsedTime(&ms, tmp.ev0, tmp.ev1));
     if (avg_ms) *avg_ms = ms / iters;
   }
+  return LSK_OK;
+}
+
+// Stand-alone attention of a batched round: attn_piece_kernel's sequence grid launched as
+// enqueue_layer launches it for lsk_round_batch.  Sequence s has seq_rows query rows at positions
+// ctx[s] - seq_rows .. ctx[s] - 1 (chunk rows s * seq_rows ..), its committed length in a DevState-strided
+// array, and its keys k / v [n_seqs][n_kv_heads][slot_positions][head_dim] in logical pages
+// [s * P, (s + 1) * P) of one pool, P = slot_positions / 64; page_perm (host, may be null) permutes the
+// logical -> physical page map of all n_seqs * P pages.
+int lsk_test_attn_seqs(const void* q, const void* k, const void* v, int32_t n_heads, int32_t n_kv_heads,
+                       int32_t head_dim, int32_t n_seqs, int32_t seq_rows, const int32_t* ctx,
+                       int32_t slot_positions, int32_t n_splits, const int32_t* page_perm, void* out) {
+  if (head_dim != 32 && head_dim != 64 && head_dim != 128) return fail(LSK_ERR_INVALID, "head_dim %d unsupported", head_dim);
+  if (!q || !k || !v || !out || !ctx || n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads || n_seqs < 1 ||
+      seq_rows < 1 || n_seqs * seq_rows > kMaxRows || n_splits < 1 || n_splits > kMaxSplits)
+    return fail(LSK_ERR_INVALID, "bad batched attention test shape");
+  if (slot_positions < kPageTokens || slot_positions % kPageTokens)
+    return fail(LSK_ERR_INVALID, "slot_positions %d is not a positive multiple of %d", slot_positions, kPageTokens);
+  for (int s = 0; s < n_seqs; ++s)
+    if (ctx[s] < seq_rows || ctx[s] > slot_positions)
+      return fail(LSK_ERR_INVALID, "sequence %d: ctx %d outside [seq_rows %d, slot %d]", s, ctx[s], seq_rows, slot_positions);
+  const int P = slot_positions / kPageTokens, n_pages = n_seqs * P;
+  std::vector<int> pth(n_pages);
+  std::vector<char> seen(n_pages, 0);
+  for (int i = 0; i < n_pages; ++i) {
+    pth[i] = page_perm ? page_perm[i] : i;
+    if (pth[i] < 0 || pth[i] >= n_pages || seen[pth[i]]) return fail(LSK_ERR_INVALID, "bad page permutation");
+    seen[pth[i]] = 1;
+  }
+  lsk_engine tmp;
+  TRY(test_engine(tmp));
+  tmp.n_splits = n_splits;
+  const int group = n_heads / n_kv_heads, rows = n_seqs * seq_rows;
+  TRY(alloc_attn_partials(&tmp, attn_bufs(n_kv_heads, group, head_dim, n_splits, rows)));
+  TRY(tmp.mem.alloc(&tmp.batch_arrive, {(size_t)n_seqs * n_kv_heads * 4, MEM_SCRATCH}, true));
+  // committed lengths DevState::len apart, the fields between them zero, as lsk_round_batch reads them
+  const int len_stride = (int)(sizeof(DevState) / sizeof(int));
+  std::vector<int> lenh((size_t)n_seqs * len_stride, 0);
+  for (int s = 0; s < n_seqs; ++s) lenh[(size_t)s * len_stride] = ctx[s] - seq_rows;
+  const size_t slot_elems = (size_t)n_kv_heads * slot_positions * head_dim;
+  __nv_bfloat16 *kp = nullptr, *vp = nullptr;
+  int *pt = nullptr, *len = nullptr;
+  TRY(tmp.mem.alloc(&kp, {slot_elems * n_seqs * 2, MEM_KV_POOL}, true));
+  TRY(tmp.mem.alloc(&vp, {slot_elems * n_seqs * 2, MEM_KV_POOL}, true));
+  TRY(tmp.mem.alloc(&pt, {(size_t)n_pages * 4, MEM_SCRATCH}));
+  TRY(tmp.mem.alloc(&len, {lenh.size() * 4, MEM_SCRATCH}));
+  CU(cudaMemcpyAsync(pt, pth.data(), (size_t)n_pages * 4, cudaMemcpyHostToDevice, tmp.stream));
+  CU(cudaMemcpyAsync(len, lenh.data(), lenh.size() * 4, cudaMemcpyHostToDevice, tmp.stream));
+  for (int s = 0; s < n_seqs; ++s) {
+    const size_t src = (size_t)s * slot_elems;
+    paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)k + src, n_kv_heads,
+                                                                  slot_positions, head_dim, pt + s * P, kp);
+    paginate_kv_kernel<<<tmp.sm_count * 4, 256, 0, tmp.stream>>>((const __nv_bfloat16*)v + src, n_kv_heads,
+                                                                  slot_positions, head_dim, pt + s * P, vp);
+  }
+  CU(cudaGetLastError());
+  const int q_cols = n_heads * head_dim;
+  AttnArgs a{};
+  a.q = (const __nv_bfloat16*)q; a.q_ld = q_cols;
+  a.out = (__nv_bfloat16*)out; a.out_ld = q_cols;
+  a.kpool = kp; a.vpool = vp; a.page_table = pt; a.base_len = len; a.pos_off = 0; a.M = seq_rows;
+  a.group = group; a.n_kv_heads = n_kv_heads; a.n_splits = n_splits;
+  a.scale = 1.0f / sqrtf((float)head_dim);
+  const AttnPieces pz{nullptr, (group * rows + 15) / 16 * 16, seq_rows, len_stride, P};
+  TRY(launch_attention(&tmp, a, head_dim, &pz, n_seqs));
+  CU(cudaStreamSynchronize(tmp.stream));
   return LSK_OK;
 }
 

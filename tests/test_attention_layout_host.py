@@ -91,3 +91,27 @@ def test_engine_raises_before_it_allocates(monkeypatch):
     arch = LlamaArch(512, 4096, 11008, 2, 32, 1, 128)
     with pytest.raises(_lib.LskError, match="group 32"):
         Engine(arch, max_ctx=256, device="cuda:0", prefill_tc=False)
+
+
+def test_batched_attention_entry_refuses_bad_shapes_before_the_device():
+    """`lsk_test_attn_seqs` checks its shape on the host: more than 16 rows, a sequence shorter than
+    its rows or longer than its slot, a slot that is not whole pages, splits outside [1, 8], a page
+    map that is not a permutation.  Without a GPU an accepted shape fails only at the device."""
+    import torch
+    lib = _lib.load()
+    dev = C.c_void_p(16)                                       # never dereferenced on a refusal
+
+    def call(n_heads=8, n_kv=2, hd=128, rows=4, ctx=(4, 300, 640), slot=640, splits=4, perm=None):
+        c = (C.c_int32 * len(ctx))(*ctx)
+        p = None if perm is None else (C.c_int32 * len(perm))(*perm)
+        return lib.lsk_test_attn_seqs(dev, dev, dev, n_heads, n_kv, hd, len(ctx), rows, c, slot, splits, p, dev)
+
+    pages = 3 * 10
+    for bad in (dict(rows=6), dict(ctx=(5,) * 17, rows=1), dict(ctx=(3, 300, 640)), dict(ctx=(4, 300, 641)),
+                dict(slot=600, ctx=(4, 300, 600)), dict(slot=0, ctx=(0, 0, 0), rows=0), dict(splits=0),
+                dict(splits=9), dict(hd=96), dict(n_heads=7), dict(perm=[0] * pages),
+                dict(perm=list(range(1, pages + 1)))):
+        assert call(**bad) == -1, bad                          # LSK_ERR_INVALID
+    if not torch.cuda.is_available():
+        assert call() == -2                                    # LSK_ERR_CUDA: the shape was accepted
+        assert call(perm=list(reversed(range(pages)))) == -2
