@@ -164,13 +164,15 @@ int lsk_round(lsk_engine* e, int32_t d_req, lsk_round_out* out);
 int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_round_out* out,
                        float* draft_conf_out);
 
-/* Batched greedy generation: n_seqs prompts share every weight pass of a round.  The batch shares
+/* Batched generation: n_seqs prompts share every weight pass of a round.  The batch shares
  * the KV pool: sequence s owns a slot of P = n_pages / n_seqs whole 64-token pages, logical pages
  * [s*P, (s+1)*P), and its position p is logical position s*64*P + p (LSK_DBG_KROW / LSK_DBG_VROW
  * read it there).  Every active sequence's round and the state it leaves are bit-identical to
  * lsk_round(e, d_seq[s]) run on that sequence alone (lsk_begin + lsk_prefill of its prompt, then the
- * same earlier rounds).  After lsk_begin with sample == 0, no_repeat_ngram_size == 0, tp_size == 1 and
- * 1 <= exit_layer <= n_layers; n_seqs in [1, max_rows].
+ * same earlier rounds; with sampling, lsk_begin with seed = seeds[s]).  After lsk_begin with
+ * no_repeat_ngram_size == 0, tp_size == 1 and 1 <= exit_layer <= n_layers; n_seqs in [1, max_rows].
+ * With sample == 1 the batch must be prefilled by lsk_prefill_batch_seeded (lsk_prefill_batch then
+ * returns LSK_ERR_INVALID).
  *
  * lsk_prefill_batch: prompt j is ids[offsets[j] .. offsets[j+1]-1] (offsets[0] == 0), length >= 1;
  * each is prefilled into its own slot exactly as lsk_prefill would prefill it alone (same routes,
@@ -184,9 +186,16 @@ int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_r
  * = n_emitted = 0 and kv_len unchanged (its rows still run, writing K/V only inside its own slot above
  * its committed length).  LSK_ERR_CTX when some sequence, active or not, has kv_len + d_req + 2 above
  * its slot's positions; LSK_ERR_STATE after any lsk_prefill or scoring call since the batch's
- * prefill.  outs: n_seqs records. */
+ * prefill.  outs: n_seqs records.
+ *
+ * lsk_prefill_batch_seeded: lsk_prefill_batch with one Philox seed per sequence (seeds: n_seqs
+ * values).  Sequence s draws, accepts and resamples exactly as a solo generation begun with seed =
+ * seeds[s], at its own step count, so a (prompt, seed) pair gives the same tokens whatever it is
+ * batched with.  A greedy generation ignores the seeds, as lsk_begin's seed. */
 int lsk_prefill_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
                       int32_t* slot_positions_out);
+int lsk_prefill_batch_seeded(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
+                             const uint64_t* seeds, int32_t* slot_positions_out);
 int lsk_round_batch(lsk_engine* e, int32_t d_req, const int32_t* d_seq, const int32_t* active,
                     lsk_round_out* outs);
 
@@ -333,7 +342,7 @@ typedef struct {
   int32_t packed_scoring;    /* lsk_score_batch or lsk_score_prefixed                             */
   int32_t tp_peer;           /* tp_size > 1: lsk_comm_init's peer region of the one-shot collectives */
   int32_t batch_seqs;        /* lsk_prefill_batch with up to this many sequences, <= 16 (any count
-                              * allocates the same buffers)                                      */
+                              * allocates the same buffers; with `sampling`, also the seeds)     */
 } lsk_memory_uses;
 /* Host-side plan of the device memory an engine with config `cfg` on a GPU with `sm_count` SMs
  * allocates at lsk_create plus for `uses` (pure host logic; works without a GPU).  The flags it

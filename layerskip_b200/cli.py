@@ -40,7 +40,7 @@ class BenchmarkArguments:             # benchmark.py:43-50
     n_shot: Optional[int] = 0
     template: Optional[str] = None
     prompt_len: int = 128             # synthetic dataset only
-    # not in the reference: generate the prompts this many at a time (greedy self-speculation only,
+    # not in the reference: generate the prompts this many at a time (self-speculation only,
     # B200SelfSpeculativeGenerationStrategy.generate_batch); 1 generates them one by one
     batch_size: int = 1
 
@@ -176,17 +176,25 @@ def _benchmark_batched(generator, examples: List[str], batch_size: int, gen_cfg:
                        warm: GenerationConfig, means: Dict[str, Mean]) -> Dict[str, Any]:
     """`benchmark` with the prompts generated batch_size at a time (generate_batch).  Each prompt's
     acceptance rate is its own; total time is the wall time of its group's generate_batch call, and
-    time per token / tokens per second count every token of the group over that time."""
+    time per token / tokens per second count every token of the group over that time.  When
+    sampling, each prompt gets its own seed, drawn in prompt order from torch's global generator as
+    a one-by-one generation draws its seed (a run under torch.manual_seed repeats)."""
     strategy = generator.generation_strategy
     if not hasattr(strategy, "generate_batch"):
         raise ValueError("--batch_size > 1 needs --generation_strategy self_speculative")
     tok = generator.tokenizer
     eos_ids = list(gen_cfg.stop_token_ids) + [tok.eos_token_id]
     ids = [tok(p, return_tensors="pt", add_special_tokens=True)["input_ids"].tolist()[0] for p in examples]
-    strategy.generate_batch(generator.model, ids[:batch_size], eos_ids, warm)
+
+    def seeds(n):
+        return [int(torch.randint(0, 2 ** 31 - 1, ()).item()) for _ in range(n)] if gen_cfg.sample else None
+
+    strategy.generate_batch(generator.model, ids[:batch_size], eos_ids, warm, seeds=seeds(len(ids[:batch_size])))
     for g in range(0, len(ids), batch_size):
+        group = ids[g:g + batch_size]
+        group_seeds = seeds(len(group))
         t0 = time.perf_counter()
-        results = strategy.generate_batch(generator.model, ids[g:g + batch_size], eos_ids, gen_cfg)
+        results = strategy.generate_batch(generator.model, group, eos_ids, gen_cfg, seeds=group_seeds)
         elapsed = time.perf_counter() - t0
         n = sum(len(r.predicted_tokens) for r in results)
         for r in results:

@@ -189,6 +189,7 @@ struct MemTable {
   MemBuf accept_rows, draft_rows;                   // per draft exit: exits_accept, exits_pd
   MemBuf batch_buf, view_table, piece_arrive;       // packed scoring
   MemBuf batch_state, batch_ctl, batch_arrive;      // batched rounds
+  MemBuf batch_seeds;                               // batched sampled rounds
   MemBuf peer_region;                               // lsk_comm_init with the one-shot collectives
 };
 
@@ -265,6 +266,8 @@ struct lsk_engine : EngineShape {
   DevState* bstate = nullptr;          // [kMaxRows] per-sequence generation state
   int* batch_ctl = nullptr;            // [2][kMaxRows] the round's d_seq, then its active flags
   unsigned int* batch_arrive = nullptr;  // [kMaxRows][kv heads] attention arrival counters
+  bool batch_seeded = false;           // the batch was prefilled with one Philox seed per sequence
+  unsigned long long* batch_seeds = nullptr;  // [kMaxRows] those seeds (sampled batches; first use)
   RoundResult* bres_host = nullptr;    // [kMaxRows] mapped pinned
   RoundResult* bres_dev = nullptr;     // device alias of bres_host
 
@@ -1162,10 +1165,19 @@ static int enqueue_round_batch(lsk_engine* e, int E, int B, int d) {
   e->cur_class = CLS_MISC;
   CU(launch(e, embed_seq_tokens_kernel, dim3(B), dim3(256), 0, embed, c.hidden, (const DevState*)e->bstate,
             e->hidden, stride));
+  const bool sample = e->gen.sample;
+  const unsigned long long* seeds = e->batch_seeds;
+  const GenParams* gp = e->gen_dev;
   for (int i = 0; i < d; ++i) {
     for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, i, B, len, i, &draft));
     TRY(enqueue_lm_head(e, i, B, i, stride));
     e->cur_class = CLS_MISC;
+    if (sample) {   // warped draft row i of sequence s -> probs_d row s * (d + 1) + i; draw and embed
+      CU(launch(e, warp_and_sample_seqs_kernel, dim3(B), dim3(kSampleThreads), 0, (const float*)e->logits,
+                e->vocab_l_pad, c.vocab, gp, (const DevState*)e->bstate, seeds, 1, d + 1, i, (int)RNG_DRAFT,
+                e->probs_d, &e->bstate->tok[1 + i], embed, c.hidden, e->hidden + (size_t)(i + 1) * c.hidden, stride));
+      continue;
+    }
     CU(launch(e, finalize_embed_seqs_kernel, dim3(8, B), dim3(128), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e),
               e->bstate, 1 + i, embed, c.hidden, e->hidden + (size_t)(i + 1) * c.hidden, stride));
   }
@@ -1173,6 +1185,15 @@ static int enqueue_round_batch(lsk_engine* e, int E, int B, int d) {
   for (int l = E; l < c.n_layers; ++l) TRY(enqueue_layer(e, l, 0, B * (d + 1), len, 0, &verify));
   TRY(enqueue_lm_head(e, 0, B * (d + 1), 0));
   e->cur_class = CLS_MISC;
+  if (sample) {
+    CU(launch(e, warp_and_sample_seqs_kernel, dim3(B * (d + 1)), dim3(kSampleThreads), 0, (const float*)e->logits,
+              e->vocab_l_pad, c.vocab, gp, (const DevState*)e->bstate, seeds, d + 1, d + 1, 0, (int)RNG_VERIFY,
+              e->probs_v, &e->bstate->verified[0], (const __nv_bfloat16*)nullptr, 0, (float*)nullptr, 0));
+    CU(launch(e, accept_sample_seqs_kernel, dim3(B), dim3(kSampleThreads), 0, e->probs_d, (const float*)e->probs_v,
+              c.vocab, d, e->bstate, gp, seeds, e->bres_dev, (const int*)e->batch_ctl,
+              (const int*)e->batch_ctl + kMaxRows));
+    return LSK_OK;
+  }
   CU(launch(e, accept_greedy_seqs_kernel, dim3(B), dim3(256), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e), d,
             e->bstate, (const GenParams*)e->gen_dev, e->bres_dev, (const int*)e->batch_ctl,
             (const int*)e->batch_ctl + kMaxRows));
@@ -1335,6 +1356,7 @@ static MemTable mem_table(const lsk_config& c, const EngineShape& s, int sm_coun
   t.batch_state = {(size_t)kMaxRows * sizeof(DevState), S};
   t.batch_ctl = {(size_t)2 * kMaxRows * 4, S};
   t.batch_arrive = {(size_t)kMaxRows * s.kv_heads_l * 4, S};
+  t.batch_seeds = {(size_t)kMaxRows * 8, S};
   t.peer_region = {peer_region_layout(c.tp_size, c.hidden).total, S};
   return t;
 }
@@ -1385,6 +1407,7 @@ static void plan_memory(const lsk_config& c, const EngineShape& s, const MemTabl
   if (u.tp_peer && c.tp_size > 1) add(t.peer_region, 1);
   if (u.batch_seqs > 0)                                // sized for max_rows sequences, whatever the batch
     for (const MemBuf& b : {t.batch_state, t.batch_ctl, t.batch_arrive}) add(b, 1);
+  if (u.batch_seqs > 0 && u.sampling) add(t.batch_seeds, 1);
 }
 
 static lsk_memory_plan plan_of(const int64_t* cat) {
@@ -2022,10 +2045,11 @@ int lsk_ar_step(lsk_engine* e, int32_t* token_out) {
   return LSK_OK;
 }
 
-// What a batch of sequences needs of the generation lsk_begin set up: greedy, no n-gram ban, one GPU,
-// a self-speculation exit layer.
-static int check_batch_generation(const lsk_engine* e) {
-  if (e->gen.sample) return fail(LSK_ERR_INVALID, "batched generation is greedy only: sampling is not supported");
+// What a batch of sequences needs of the generation lsk_begin set up: greedy, or sampling with one seed
+// per sequence (`seeded`); no n-gram ban, one GPU, a self-speculation exit layer.
+static int check_batch_generation(const lsk_engine* e, bool seeded) {
+  if (e->gen.sample && !seeded)
+    return fail(LSK_ERR_INVALID, "batched sampling needs one seed per sequence: use lsk_prefill_batch_seeded");
   if (e->gen.no_repeat_ngram_size > 0)
     return fail(LSK_ERR_INVALID, "batched generation does not support the n-gram ban (no_repeat_ngram_size %d)",
                 e->gen.no_repeat_ngram_size);
@@ -2040,11 +2064,12 @@ static int check_batch_generation(const lsk_engine* e) {
 // its position p is logical position s * 64 * P + p.
 static int batch_slot_positions(const lsk_engine* e, int n) { return e->n_pages / n * kPageTokens; }
 
-int lsk_prefill_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
-                      int32_t* slot_positions_out) {
+// lsk_prefill_batch (seeds == NULL) and lsk_prefill_batch_seeded
+static int prefill_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
+                         const uint64_t* seeds, int32_t* slot_positions_out) {
   if (!e || !ids || !offsets) return fail(LSK_ERR_INVALID, "null argument");
   if (!e->began) return fail(LSK_ERR_STATE, "lsk_begin must precede lsk_prefill_batch");
-  TRY(check_batch_generation(e));
+  TRY(check_batch_generation(e, seeds != nullptr));
   if (n_seqs < 1 || n_seqs > e->max_rows)
     return fail(LSK_ERR_INVALID, "n_seqs %d outside [1, %d]", n_seqs, e->max_rows);
   if (offsets[0] != 0) return fail(LSK_ERR_INVALID, "offsets[0] must be 0 (got %d)", offsets[0]);
@@ -2070,11 +2095,15 @@ int lsk_prefill_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets,
     memset(e->bres_host, 0, kMaxRows * sizeof(RoundResult));
     CU(cudaHostGetDevicePointer((void**)&e->bres_dev, e->bres_host, 0));
   }
+  if (e->gen.sample) TRY(alloc_once(e, &e->batch_seeds, t.batch_seeds));
   e->prefilled = false;
   e->batch_n = 0;
   e->host_len = 0;
   CU(cudaEventRecord(e->ev0, e->stream));
   CU(cudaMemsetAsync(e->bstate, 0, t.batch_state.bytes, e->stream));
+  // the rounds' graphs read the seeds from here: one captured graph serves every set of seeds
+  if (e->gen.sample)
+    CU(cudaMemcpyAsync(e->batch_seeds, seeds, (size_t)n_seqs * sizeof(uint64_t), cudaMemcpyHostToDevice, e->stream));
   // prompt j through lsk_prefill's route, over its slot's page-table view
   int* const table = e->page_table;
   for (int j = 0; j < n_seqs; ++j) {
@@ -2094,15 +2123,27 @@ int lsk_prefill_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets,
   e->batch_len.assign(n_seqs, 0);
   for (int j = 0; j < n_seqs; ++j) e->batch_len[j] = offsets[j + 1] - offsets[j] - 1;
   e->batch_n = n_seqs;
+  e->batch_seeded = seeds != nullptr;
   if (slot_positions_out) *slot_positions_out = slot;
   return LSK_OK;
+}
+
+int lsk_prefill_batch(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
+                      int32_t* slot_positions_out) {
+  return prefill_batch(e, ids, offsets, n_seqs, nullptr, slot_positions_out);
+}
+
+int lsk_prefill_batch_seeded(lsk_engine* e, const int32_t* ids, const int32_t* offsets, int32_t n_seqs,
+                             const uint64_t* seeds, int32_t* slot_positions_out) {
+  if (!seeds) return fail(LSK_ERR_INVALID, "null argument");
+  return prefill_batch(e, ids, offsets, n_seqs, seeds, slot_positions_out);
 }
 
 int lsk_round_batch(lsk_engine* e, int32_t d_req, const int32_t* d_seq, const int32_t* active,
                     lsk_round_out* outs) {
   if (!e || !outs) return fail(LSK_ERR_INVALID, "null argument");
   if (!e->batch_n) return fail(LSK_ERR_STATE, "lsk_prefill_batch must precede lsk_round_batch");
-  TRY(check_batch_generation(e));
+  TRY(check_batch_generation(e, e->batch_seeded));
   const int B = e->batch_n, E = e->gen.exit_layer;
   if (d_req < 0 || B * (d_req + 1) > e->max_rows)
     return fail(LSK_ERR_INVALID, "%d sequences x (d_req %d + 1) rows exceed the %d rows of a step", B, d_req,
@@ -2120,7 +2161,8 @@ int lsk_round_batch(lsk_engine* e, int32_t d_req, const int32_t* d_seq, const in
       return fail(LSK_ERR_CTX, "sequence %d: context %d + %d exceeds its slot of %d positions", s, e->batch_len[s],
                   d_req + 1, slot);
   CU(cudaMemcpyAsync(e->batch_ctl, ctl, sizeof(ctl), cudaMemcpyHostToDevice, e->stream));
-  const long long key = ((long long)E << 20) | ((long long)d_req << 8) | 16 | 1 | ((long long)B << 40);
+  const long long key = ((long long)E << 20) | ((long long)d_req << 8) | (e->gen.sample ? 4 : 0) | 16 | 1 |
+                        ((long long)B << 40);
   TRY(run_cached(e, key, [&]() { return enqueue_round_batch(e, E, B, d_req); }));
   for (int s = 0; s < B; ++s) {
     copy_result(e->bres_host[s], &outs[s]);

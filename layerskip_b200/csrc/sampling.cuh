@@ -34,6 +34,12 @@ __device__ __forceinline__ float rng_uniform(const GenParams& gp, int step, int 
                                 make_uint2((uint32_t)gp.seed, (uint32_t)(gp.seed >> 32)));
   return u01(r.x);
 }
+// The same draw with the key given explicitly: batched rounds key each sequence by its own seed.
+__device__ __forceinline__ float rng_uniform(unsigned long long seed, int step, int row, int purpose) {
+  const uint4 r = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)row, (uint32_t)purpose, 0x4c534bu),
+                                make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+  return u01(r.x);
+}
 
 // ---- block-wide helpers (blockDim.x == kSampleThreads), deterministic order
 __device__ __forceinline__ float block_sum(float v, float* red) {
@@ -409,6 +415,126 @@ accept_sample_kernel(const float* __restrict__ p_draft, const float* __restrict_
     res->kv_len = st->len;
     __threadfence_system();
     *reinterpret_cast<volatile int*>(&res->seq) = seq;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Batched sampled rounds (lsk_round_batch after lsk_prefill_batch_seeded).  Sequence s owns rows
+// s * seq_rows .. s * seq_rows + seq_rows - 1 of probs_d / probs_v (seq_rows = d + 1) and draws
+// with its own seed seeds[s] at its own step count, with the counters a round of that sequence
+// alone uses, so each sequence's draws do not depend on the rest of the batch.
+// ---------------------------------------------------------------------------------------------
+// warp_and_sample_kernel for several sequences: CTA r serves sequence s = r / rows_per_seq and its
+// row j = r % rows_per_seq.  It warps logits row r, writes the warped row to probs row
+// s * seq_rows + row_base + j, draws with counter (st[s].step_count, row_base + j, purpose) into
+// tok_out[s * (DevState ints) + j] (tok_out points into st[0]) and, when `embed` is set, embeds
+// the token into emb_rows + s * emb_ld.
+//   draft step i: grid B, rows_per_seq 1, row_base i, tok_out &st[0].tok[1 + i];
+//   verify:       grid B * seq_rows, rows_per_seq seq_rows, row_base 0, tok_out &st[0].verified[0].
+__global__ void __launch_bounds__(kSampleThreads)
+warp_and_sample_seqs_kernel(const float* __restrict__ logits, int ld, int V,
+                            const GenParams* __restrict__ gpp, const DevState* __restrict__ st,
+                            const unsigned long long* __restrict__ seeds, int rows_per_seq, int seq_rows,
+                            int row_base, int purpose, float* __restrict__ probs, int* __restrict__ tok_out,
+                            const __nv_bfloat16* __restrict__ embed, int hidden,
+                            float* __restrict__ emb_rows, int emb_ld) {
+  __shared__ float red[96 + 32];
+  __shared__ uint32_t hist[512];
+  __shared__ uint32_t s_prefix;
+  __shared__ float s_g;
+  __shared__ int s_pick;
+  pdl_launch_dependents();
+  pdl_wait();
+  const GenParams gp = *gpp;
+  const int r = blockIdx.x;
+  const int s = r / rows_per_seq, j = r - s * rows_per_seq;
+  float* pr = probs + ((size_t)s * seq_rows + row_base + j) * V;
+  warp_row(logits + (size_t)r * ld, V, gp.temperature, gp.top_k, gp.top_p, pr, red, hist, s_prefix, s_g);
+  const float u = rng_uniform(seeds[s], st[s].step_count, row_base + j, purpose);
+  const int tok = block_sample_index(pr, V, u, red, &s_pick);
+  if (threadIdx.x == 0) tok_out[(size_t)s * (sizeof(DevState) / sizeof(int)) + j] = tok;
+  if (embed != nullptr) embed_row(embed, hidden, tok, emb_rows + (size_t)s * emb_ld, threadIdx.x, blockDim.x);
+}
+
+// accept_sample_kernel for a batch: CTA s serves sequence s, whose drafts are rows s * (d + 1) .. of
+// probs_d and verify rows the same rows of probs_v.  An active sequence runs the rejection test and
+// residual resample with its own seed and d_seq[s] as d_stop (as accept_greedy_seqs_kernel), and
+// commits into st[s] / res[s]; its residual goes to probs_d row s * (d + 1) + d, which no draft
+// writes.  An inactive sequence commits nothing and reports no tokens.  The body restates
+// accept_sample_kernel's rather than sharing it: routing that kernel through a common function
+// changes its instructions.
+__global__ void __launch_bounds__(kSampleThreads)
+accept_sample_seqs_kernel(float* __restrict__ probs_d, const float* __restrict__ probs_v, int V, int d,
+                          DevState* __restrict__ sts, const GenParams* __restrict__ gpp,
+                          const unsigned long long* __restrict__ seeds, RoundResult* __restrict__ ress,
+                          const int* __restrict__ d_seq, const int* __restrict__ active) {
+  __shared__ float red[96 + 32];
+  __shared__ int s_pick;
+  __shared__ int s_n, s_dact, s_reject;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int s = blockIdx.x;
+  DevState* st = &sts[s];
+  RoundResult* res = &ress[s];
+  if (!active[s]) {
+    if (threadIdx.x == 0) {
+      res->n_drafted = res->n_matches = res->n_emitted = 0;
+      res->kv_len = st->len;
+      __threadfence_system();
+      *reinterpret_cast<volatile int*>(&res->seq) = 0;
+    }
+    return;
+  }
+  const GenParams gp = *gpp;
+  const unsigned long long seed = seeds[s];
+  const float* p_draft = probs_d + (size_t)s * (d + 1) * V;
+  const float* p_verify = probs_v + (size_t)s * (d + 1) * V;
+  if (threadIdx.x == 0) {
+    const int d_lim = d_seq[s];
+    int d_act = d_lim;
+    for (int i = 0; i < d_lim; ++i)
+      if (is_eos(gp, st->tok[1 + i])) { d_act = i + 1; break; }
+    int n = 0, reject = -1;
+    for (int i = 0; i < d_act; ++i) {
+      const int t = st->tok[1 + i];
+      const float pv = p_verify[(size_t)i * V + t], pd = p_draft[(size_t)i * V + t];
+      const float u = rng_uniform(seed, st->step_count, i, RNG_ACCEPT);
+      if (u < fminf(1.0f, pv / pd)) ++n;
+      else { reject = i; break; }
+    }
+    s_n = n; s_dact = d_act; s_reject = reject;
+  }
+  __syncthreads();
+  const int n = s_n, d_act = s_dact, reject = s_reject;
+  int bonus;
+  if (reject >= 0) {
+    // resample from norm(max(p_v - p_d, 0))   (max_fn, :27-29)
+    float* scratch = probs_d + ((size_t)s * (d + 1) + d) * V;
+    const float* pv = p_verify + (size_t)reject * V;
+    const float* pd = p_draft + (size_t)reject * V;
+    for (int j = threadIdx.x; j < V; j += kSampleThreads) scratch[j] = fmaxf(pv[j] - pd[j], 0.f);
+    __syncthreads();
+    const float u = rng_uniform(seed, st->step_count, reject, RNG_RESID);
+    bonus = block_sample_index(scratch, V, u, red, &s_pick);
+  } else {
+    bonus = st->verified[n];             // the verifier's own draw at row n (= d_act)
+  }
+  if (threadIdx.x == 0) {
+    res->n_drafted = d_act;
+    res->n_matches = n;
+    res->n_emitted = n + 1;
+    for (int i = 0; i < d_act; ++i) res->draft_ids[i] = st->tok[1 + i];
+    for (int i = 0; i <= d_act; ++i) res->verified_ids[i] = st->verified[i];
+    res->verified_ids[n] = bonus;
+    for (int i = 0; i < n; ++i) res->emitted_ids[i] = st->tok[1 + i];
+    res->emitted_ids[n] = bonus;
+    st->len += n + 1;
+    st->n_out += n + 1;
+    st->tok[0] = bonus;
+    st->step_count += 1;
+    res->kv_len = st->len;
+    __threadfence_system();
+    *reinterpret_cast<volatile int*>(&res->seq) = 0;
   }
 }
 

@@ -213,11 +213,19 @@ class Engine:
             kv_len=out.kv_len)
 
     # ------------------------------------------------------------------ batched generation
-    def prefill_batch(self, prompts: Sequence[Sequence[int]]) -> int:
-        """Prefill every prompt into its own slot of the KV pool (after `begin`, greedy, no n-gram ban,
-        one GPU).  Returns the positions each slot holds: `batch_slot_positions(max_ctx, len(prompts))`.
-        Each prompt is prefilled exactly as `prefill` would prefill it alone."""
+    def prefill_batch(self, prompts: Sequence[Sequence[int]], seeds: Optional[Sequence[int]] = None) -> int:
+        """Prefill every prompt into its own slot of the KV pool (after `begin`, no n-gram ban, one
+        GPU).  Returns the positions each slot holds: `batch_slot_positions(max_ctx, len(prompts))`.
+        Each prompt is prefilled exactly as `prefill` would prefill it alone.  A sampled generation
+        needs `seeds`, one Philox seed in [0, 2**64) per prompt: sequence s then samples as a solo
+        generation begun with `seed=seeds[s]`.  Greedy generation ignores the seeds."""
         prompts = [[int(t) for t in p] for p in prompts]
+        if seeds is not None:
+            seeds = [int(x) for x in seeds]
+            if len(seeds) != len(prompts):
+                raise ValueError(f"{len(seeds)} seeds for {len(prompts)} prompts")
+            if any(not 0 <= x < 2 ** 64 for x in seeds):
+                raise ValueError("seeds must be in [0, 2**64)")
         offsets = [0]
         for p in prompts:
             offsets.append(offsets[-1] + len(p))
@@ -226,7 +234,11 @@ class Engine:
         off = (C.c_int32 * len(offsets))(*offsets)
         slot = C.c_int32()
         with torch.cuda.device(self.device):
-            _lib.check(self._lib.lsk_prefill_batch(self._h, arr, off, len(prompts), C.byref(slot)))
+            if seeds is None:
+                _lib.check(self._lib.lsk_prefill_batch(self._h, arr, off, len(prompts), C.byref(slot)))
+            else:
+                sd = (C.c_uint64 * max(len(seeds), 1))(*seeds)
+                _lib.check(self._lib.lsk_prefill_batch_seeded(self._h, arr, off, len(prompts), sd, C.byref(slot)))
         self._batch_n = len(prompts)
         return slot.value
 

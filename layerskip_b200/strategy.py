@@ -177,17 +177,23 @@ class B200SelfSpeculativeGenerationStrategy(GenerationStrategy):
 
     def generate_batch(self, model, prompts: List[List[int]], eos_token_ids: List[int],
                        generation_config: GenerationConfig, logits_processors=None, stopping_criteria=None,
-                       streamer=None) -> List[GenerationStrategyResult]:
-        """Greedy self-speculative generation of several prompts at once: every round runs all the
+                       streamer=None, seeds: Optional[List[int]] = None) -> List[GenerationStrategyResult]:
+        """Self-speculative generation of several prompts at once: every round runs all the
         sequences still generating through the same weight passes (`Engine.round_batch`).  Result j
         equals `generate_token_ids(model, prompts[j], ...)` with the same config: the outer loop
         below is the reference's, per sequence (max_steps clamp, acceptance accounting, EOS
-        truncation), and each sequence's rounds are bit-identical to its rounds alone.  Sampling,
-        logits processors, stopping criteria and streamers are not supported here.  The prompts share
+        truncation), and each sequence's rounds are bit-identical to its rounds alone.  Sampling
+        (`cfg.sample`) needs `seeds`, one per prompt in [0, 2**64): prompt j then samples as
+        `generate_token_ids` does with the engine seed `seeds[j]`, whatever it is batched with.
+        Logits processors, stopping criteria and streamers are not supported here.  The prompts share
         the KV pool: each gets ceil(max_ctx / 64) // len(prompts) whole 64-token pages."""
         cfg = generation_config
-        if cfg.sample:
-            raise NotImplementedError("generate_batch is greedy only: set sample=False")
+        if cfg.sample and seeds is None:
+            raise NotImplementedError("generate_batch without seeds is greedy only: set sample=False, or pass "
+                                      "one seed per prompt to sample")
+        if cfg.sample and (len(seeds) != len(prompts) or any(not 0 <= int(x) < 2 ** 64 for x in seeds)):
+            raise ValueError(f"sampling needs one seed in [0, 2**64) per prompt ({len(seeds)} seeds for "
+                             f"{len(prompts)} prompts)")
         if logits_processors or cfg.no_repeat_ngram_size:
             raise NotImplementedError("generate_batch supports no logits processors (no n-gram ban)")
         if stopping_criteria or cfg.stop_words:
@@ -213,8 +219,9 @@ class B200SelfSpeculativeGenerationStrategy(GenerationStrategy):
             raise ValueError(f"the longest prompt + max_steps ({cfg.max_steps}) + num_speculations ({D}) + 1 needs "
                              f"{need} KV positions but each of {n} prompts gets {slot} (max_ctx={eng.max_ctx}); "
                              "construct the strategy with a larger max_ctx or generate fewer prompts at once")
-        eng.begin(exit_layer=cfg.exit_layer, max_steps=cfg.max_steps, eos_token_ids=eos_token_ids, sample=False)
-        eng.prefill_batch(prompts)
+        eng.begin(exit_layer=cfg.exit_layer, max_steps=cfg.max_steps, eos_token_ids=eos_token_ids,
+                  sample=cfg.sample, temperature=cfg.temperature, top_k=cfg.top_k, top_p=cfg.top_p)
+        eng.prefill_batch(prompts, seeds if cfg.sample else None)
         outs: List[List[int]] = [[] for _ in prompts]
         matches, drafted = [0] * n, [0] * n
         active = [cfg.max_steps > 0] * n

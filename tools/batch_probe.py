@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Batched greedy self-speculation: aggregate throughput of B prompts generated together.
+"""Batched self-speculation: aggregate throughput of B prompts generated together.
 
 Synthetic Llama-2-7B with layers >= E damped by alpha (the bench's model family), E = 8, greedy
 generations of the bench's prompts.  For B = 1, 2, 4, 8, 16 with D = 16 / B - 1 drafts (so every
@@ -8,9 +8,11 @@ verify carries 16 rows), B prompts run together through `Engine.round_batch` (B 
 deactivation).  Per B it reports aggregate tokens/s over the whole generation (wall time, prefill
 included), rounds/s, mean device ms per round and the acceptance rate (matches / drafts).  Every B
 runs once untimed first (graph capture of every round shape).  Prints the GPU name and power limit
-first (read-only nvidia-smi query), then one JSON line per B.
+first (read-only nvidia-smi query), then one JSON line per B.  With --sample each B runs greedy and
+then sampled (temperature 0.6, top-p 0.9, the reference's defaults; sequence s seeded with 1000 + s),
+one JSON line per mode.
 
-    python tools/batch_probe.py [--batches 1,2,4,8,16] [--alpha 0.3] [--max_steps 128]
+    python tools/batch_probe.py [--batches 1,2,4,8,16] [--alpha 0.3] [--max_steps 128] [--sample]
 """
 import argparse
 import json
@@ -24,13 +26,18 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from score_probe import gpu_name_and_power_limit  # noqa: E402
 
 
-def generate(eng, prompts, eos, exit_layer, max_steps, D):
-    """Greedy generation of `prompts` together; returns (outputs, device ms per round, drafts, matches)."""
-    eng.begin(exit_layer=exit_layer, max_steps=max_steps, eos_token_ids=eos, sample=False)
+SAMPLING = dict(temperature=0.6, top_k=0, top_p=0.9)
+
+
+def generate(eng, prompts, eos, exit_layer, max_steps, D, sample=False):
+    """Generation of `prompts` together; returns (outputs, device ms per round, drafts, matches)."""
+    seeds = [1000 + s for s in range(len(prompts))]
+    eng.begin(exit_layer=exit_layer, max_steps=max_steps, eos_token_ids=eos, sample=sample,
+              seed=seeds[0], **SAMPLING)
     if len(prompts) == 1:
         eng.prefill(prompts[0])
     else:
-        eng.prefill_batch(prompts)
+        eng.prefill_batch(prompts, seeds if sample else None)
     outs = [[] for _ in prompts]
     active = [True] * len(prompts)
     ms, drafted, matched = [], 0, 0
@@ -61,6 +68,7 @@ def main():
     ap.add_argument("--batches", default="1,2,4,8,16")
     ap.add_argument("--prompt_len", type=int, default=128)
     ap.add_argument("--max_steps", type=int, default=128)
+    ap.add_argument("--sample", action="store_true", help="also run each B sampled (T 0.6, top-p 0.9)")
     a = ap.parse_args()
     import torch
     from layerskip_b200.engine import Engine
@@ -79,19 +87,21 @@ def main():
                       "alpha": a.alpha, "prompt_len": a.prompt_len, "max_steps": a.max_steps,
                       "max_rows": eng.max_rows}), flush=True)
     for B in batches:
-        D = eng.max_rows // B - 1
-        group = prompts[:B]
-        generate(eng, group, eos, a.exit_layer, a.max_steps, D)          # warm-up: capture every shape
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        outs, ms, drafted, matched = generate(eng, group, eos, a.exit_layer, a.max_steps, D)
-        s = time.perf_counter() - t0
-        tokens = sum(len(o) for o in outs)
-        print(json.dumps({"B": B, "D": D, "tokens": tokens, "seconds": round(s, 4),
-                          "tokens_per_s": round(tokens / s, 1), "rounds": len(ms),
-                          "rounds_per_s": round(len(ms) / s, 1),
-                          "device_ms_per_round": round(sum(ms) / len(ms), 4),
-                          "acceptance": round(matched / drafted, 4) if drafted else None}), flush=True)
+        for sample in ((False, True) if a.sample else (False,)):
+            D = eng.max_rows // B - 1
+            group = prompts[:B]
+            generate(eng, group, eos, a.exit_layer, a.max_steps, D, sample)  # warm-up: capture every shape
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            outs, ms, drafted, matched = generate(eng, group, eos, a.exit_layer, a.max_steps, D, sample)
+            s = time.perf_counter() - t0
+            tokens = sum(len(o) for o in outs)
+            print(json.dumps({"B": B, "D": D, "mode": "sampled" if sample else "greedy", "tokens": tokens,
+                              "seconds": round(s, 4),
+                              "tokens_per_s": round(tokens / s, 1), "rounds": len(ms),
+                              "rounds_per_s": round(len(ms) / s, 1),
+                              "device_ms_per_round": round(sum(ms) / len(ms), 4),
+                              "acceptance": round(matched / drafted, 4) if drafted else None}), flush=True)
     eng.close()
 
 
