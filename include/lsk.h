@@ -199,6 +199,23 @@ int lsk_prefill_batch_seeded(lsk_engine* e, const int32_t* ids, const int32_t* o
 int lsk_round_batch(lsk_engine* e, int32_t d_req, const int32_t* d_seq, const int32_t* active,
                     lsk_round_out* outs);
 
+/* lsk_round_batch with confidence-threshold drafting (lsk_round_adaptive's stop rule) for every
+ * sequence: d_max takes d_req's place, and sequence s stops drafting after draft j when that draft is
+ * an EOS, when its confidence is below min_confidence (one threshold for the whole batch), or when
+ * j + 1 == d_seq[s].  Draft step j >= 1 runs (graph mode) iff some active sequence has not stopped
+ * before it; a sequence that stopped still has its rows computed while others draft on, causally
+ * invisible to its kept rows.  Every active sequence's round, confidences and committed K/V rows are
+ * bit-identical to lsk_round_adaptive(e, d_seq[s], min_confidence) of that sequence alone (and so to
+ * lsk_round(e, n_drafted)); an inactive one behaves as in lsk_round_batch.  min_confidence == 0 gives
+ * lsk_round_batch(e, d_max, d_seq, active); d_max == 0 is lsk_round_batch(e, 0, ...).
+ * LSK_FLAG_NO_GRAPH runs every draft step, with the same results.
+ * draft_conf_out (host, may be NULL): [n_seqs][LSK_MAX_SPEC] floats; sequence s receives the
+ * confidences of its outs[s].n_drafted kept drafts.
+ * Same preconditions, state rules and errors as lsk_round_batch; also LSK_ERR_INVALID for
+ * min_confidence outside [0, 1] or NaN. */
+int lsk_round_batch_adaptive(lsk_engine* e, int32_t d_max, const int32_t* d_seq, const int32_t* active,
+                             float min_confidence, lsk_round_out* outs, float* draft_conf_out);
+
 /* One autoregressive step on the same engine (autoregressive_generator.py:44-67): all layers, or
  * layers < E when the generation's exit_layer > 0.  Returns the chosen token; the caller decides
  * about EOS exactly as the reference does (:66-67). */
@@ -336,13 +353,14 @@ typedef struct {
   int32_t lm_head_tc;        /* the opt-in wgmma LM head was asked for (LSK_LMHEAD_TC=1)          */
   int32_t sampling;          /* lsk_begin with sample = 1                                         */
   int32_t ngram_ban;         /* lsk_begin with no_repeat_ngram_size > 0                           */
-  int32_t adaptive;          /* lsk_round_adaptive                                                */
+  int32_t adaptive;          /* lsk_round_adaptive (lsk_round_batch_adaptive with batch_seqs)     */
   int32_t score_exits;       /* scoring with up to this many exits (lsk_score: 1), <= LSK_MAX_EXITS */
   int32_t accept_exits;      /* lsk_score_exits with accept_out, up to this many exits            */
   int32_t packed_scoring;    /* lsk_score_batch or lsk_score_prefixed                             */
   int32_t tp_peer;           /* tp_size > 1: lsk_comm_init's peer region of the one-shot collectives */
   int32_t batch_seqs;        /* lsk_prefill_batch with up to this many sequences, <= 16 (any count
-                              * allocates the same buffers; with `sampling`, also the seeds)     */
+                              * allocates the same buffers; with `sampling`, also the seeds; with
+                              * `adaptive`, also lsk_round_batch_adaptive's confidence scratch)   */
 } lsk_memory_uses;
 /* Host-side plan of the device memory an engine with config `cfg` on a GPU with `sm_count` SMs
  * allocates at lsk_create plus for `uses` (pure host logic; works without a GPU).  The flags it

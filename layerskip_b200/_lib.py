@@ -113,6 +113,8 @@ SIGNATURES = {
                                            C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]),
     "lsk_round_batch": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                   C.POINTER(lsk_round_out)]),
+    "lsk_round_batch_adaptive": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                           C.c_float, C.POINTER(lsk_round_out), C.POINTER(C.c_float)]),
     "lsk_ar_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "lsk_score": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32,
                             C.POINTER(C.c_float), C.POINTER(C.c_int32)]),

@@ -190,6 +190,7 @@ struct MemTable {
   MemBuf batch_buf, view_table, piece_arrive;       // packed scoring
   MemBuf batch_state, batch_ctl, batch_arrive;      // batched rounds
   MemBuf batch_seeds;                               // batched sampled rounds
+  MemBuf conf_seqs;                                 // batched adaptive rounds
   MemBuf peer_region;                               // lsk_comm_init with the one-shot collectives
 };
 
@@ -279,6 +280,7 @@ struct lsk_engine : EngineShape {
   cudaStream_t stream = nullptr;
   cudaStream_t body_stream = nullptr;  // captures the bodies of an adaptive round's conditional nodes
   ConfScratch* conf_scratch = nullptr; // draft_confidence_kernel's partials and arrival counter
+  ConfSeqsScratch* conf_seqs = nullptr;  // draft_confidence_seqs_kernel's partials, counters, d_stop, threshold
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::map<long long, cudaGraphExec_t> graphs;
   ncclComm_t comm = nullptr;
@@ -1153,51 +1155,125 @@ static int enqueue_round_adaptive(lsk_engine* e, int E, int d) {
 // B * (d + 1) rows, each sequence at its own positions, over its own KV slot (page-table view
 // page_table + s * P).  The GEMMs are batch-invariant and the attention partition is fixed by
 // absolute key index, so every row is computed as in a round of that sequence alone.
-static int enqueue_round_batch(lsk_engine* e, int E, int B, int d) {
+struct BatchRows {
+  SeqRows draft, verify;
+  int stride;                          // floats between two sequences' rows of one draft step
+};
+static BatchRows batch_rows(lsk_engine* e, int B, int d) {
   const lsk_config& c = e->cfg;
-  const int* len = &e->bstate->len;
   const int len_stride = (int)(sizeof(DevState) / sizeof(int));
   const int P = e->n_pages / B;
   const int stride = (d + 1) * c.hidden;
-  const SeqRows draft{B, 1, len_stride, P, stride};
-  const SeqRows verify{B, d + 1, len_stride, P, c.hidden};
-  const __nv_bfloat16* embed = e->embed;
+  return {SeqRows{B, 1, len_stride, P, stride}, SeqRows{B, d + 1, len_stride, P, c.hidden}, stride};
+}
+
+// Draft step i's head on row i of every sequence; each sequence's token becomes its tok[1 + i] and is
+// embedded into its row i + 1 (sampling: the warped row goes to probs_d row s * (d + 1) + i).
+static int enqueue_draft_token_seqs(lsk_engine* e, int i, int B, int d, int stride) {
+  const lsk_config& c = e->cfg;
+  TRY(enqueue_lm_head(e, i, B, i, stride));
   e->cur_class = CLS_MISC;
-  CU(launch(e, embed_seq_tokens_kernel, dim3(B), dim3(256), 0, embed, c.hidden, (const DevState*)e->bstate,
-            e->hidden, stride));
-  const bool sample = e->gen.sample;
-  const unsigned long long* seeds = e->batch_seeds;
-  const GenParams* gp = e->gen_dev;
-  for (int i = 0; i < d; ++i) {
-    for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, i, B, len, i, &draft));
-    TRY(enqueue_lm_head(e, i, B, i, stride));
-    e->cur_class = CLS_MISC;
-    if (sample) {   // warped draft row i of sequence s -> probs_d row s * (d + 1) + i; draw and embed
-      CU(launch(e, warp_and_sample_seqs_kernel, dim3(B), dim3(kSampleThreads), 0, (const float*)e->logits,
-                e->vocab_l_pad, c.vocab, gp, (const DevState*)e->bstate, seeds, 1, d + 1, i, (int)RNG_DRAFT,
-                e->probs_d, &e->bstate->tok[1 + i], embed, c.hidden, e->hidden + (size_t)(i + 1) * c.hidden, stride));
-      continue;
-    }
-    CU(launch(e, finalize_embed_seqs_kernel, dim3(8, B), dim3(128), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e),
-              e->bstate, 1 + i, embed, c.hidden, e->hidden + (size_t)(i + 1) * c.hidden, stride));
+  if (e->gen.sample) {
+    CU(launch(e, warp_and_sample_seqs_kernel, dim3(B), dim3(kSampleThreads), 0, (const float*)e->logits,
+              e->vocab_l_pad, c.vocab, (const GenParams*)e->gen_dev, (const DevState*)e->bstate,
+              (const unsigned long long*)e->batch_seeds, 1, d + 1, i, (int)RNG_DRAFT, e->probs_d,
+              &e->bstate->tok[1 + i], (const __nv_bfloat16*)e->embed, c.hidden,
+              e->hidden + (size_t)(i + 1) * c.hidden, stride));
+    return LSK_OK;
   }
-  for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, d, B, len, d, &draft));
-  for (int l = E; l < c.n_layers; ++l) TRY(enqueue_layer(e, l, 0, B * (d + 1), len, 0, &verify));
+  CU(launch(e, finalize_embed_seqs_kernel, dim3(8, B), dim3(128), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e),
+            e->bstate, 1 + i, (const __nv_bfloat16*)e->embed, c.hidden, e->hidden + (size_t)(i + 1) * c.hidden,
+            stride));
+  return LSK_OK;
+}
+
+// The batch's verify after the draft rows: layers >= E on all B * (d + 1) rows, the head, and the
+// accept, which keeps d_stop[s] drafts of active sequence s (lsk_round_batch: d_seq).
+static int enqueue_verify_seqs(lsk_engine* e, int E, int B, int d, const BatchRows& rows, const int* d_stop) {
+  const lsk_config& c = e->cfg;
+  const int* len = &e->bstate->len;
+  const int* active = (const int*)e->batch_ctl + kMaxRows;
+  const GenParams* gp = e->gen_dev;
+  for (int l = E; l < c.n_layers; ++l) TRY(enqueue_layer(e, l, 0, B * (d + 1), len, 0, &rows.verify));
   TRY(enqueue_lm_head(e, 0, B * (d + 1), 0));
   e->cur_class = CLS_MISC;
-  if (sample) {
+  if (e->gen.sample) {
+    const unsigned long long* seeds = e->batch_seeds;
     CU(launch(e, warp_and_sample_seqs_kernel, dim3(B * (d + 1)), dim3(kSampleThreads), 0, (const float*)e->logits,
               e->vocab_l_pad, c.vocab, gp, (const DevState*)e->bstate, seeds, d + 1, d + 1, 0, (int)RNG_VERIFY,
               e->probs_v, &e->bstate->verified[0], (const __nv_bfloat16*)nullptr, 0, (float*)nullptr, 0));
     CU(launch(e, accept_sample_seqs_kernel, dim3(B), dim3(kSampleThreads), 0, e->probs_d, (const float*)e->probs_v,
-              c.vocab, d, e->bstate, gp, seeds, e->bres_dev, (const int*)e->batch_ctl,
-              (const int*)e->batch_ctl + kMaxRows));
+              c.vocab, d, e->bstate, gp, seeds, e->bres_dev, d_stop, active));
     return LSK_OK;
   }
   CU(launch(e, accept_greedy_seqs_kernel, dim3(B), dim3(256), 0, cand_val_ptr(e), cand_idx_ptr(e), n_cand(e), d,
-            e->bstate, (const GenParams*)e->gen_dev, e->bres_dev, (const int*)e->batch_ctl,
-            (const int*)e->batch_ctl + kMaxRows));
+            e->bstate, gp, e->bres_dev, d_stop, active));
   return LSK_OK;
+}
+
+static int enqueue_round_batch(lsk_engine* e, int E, int B, int d) {
+  const lsk_config& c = e->cfg;
+  const int* len = &e->bstate->len;
+  const BatchRows rows = batch_rows(e, B, d);
+  e->cur_class = CLS_MISC;
+  CU(launch(e, embed_seq_tokens_kernel, dim3(B), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
+            (const DevState*)e->bstate, e->hidden, rows.stride));
+  for (int i = 0; i < d; ++i) {
+    for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, i, B, len, i, &rows.draft));
+    TRY(enqueue_draft_token_seqs(e, i, B, d, rows.stride));
+  }
+  for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, d, B, len, d, &rows.draft));
+  return enqueue_verify_seqs(e, E, B, d, rows, (const int*)e->batch_ctl);
+}
+
+// Confidences and stop rules of draft step j for every sequence (draft_confidence_seqs_kernel).
+static int emit_draft_confidence_seqs(lsk_engine* e, int j, int B, int d, cudaGraphConditionalHandle next,
+                                      bool has_next) {
+  const lsk_config& c = e->cfg;
+  e->cur_class = CLS_MISC;
+  const bool sample = e->gen.sample;
+  const int grid = sample ? 1 : std::min(kConfMaxCtas, (c.vocab + kConfCols - 1) / kConfCols);
+  CU(launch(e, draft_confidence_seqs_kernel, dim3(grid, B), dim3(kConfThreads), 0,
+            sample ? (const float*)nullptr : (const float*)e->logits, e->vocab_l_pad,
+            sample ? (const float*)e->probs_d : (const float*)nullptr, c.vocab, d + 1, e->bstate,
+            (const GenParams*)e->gen_dev, e->bres_dev, e->conf_seqs, (const int*)e->batch_ctl,
+            (const int*)e->batch_ctl + kMaxRows, j, e->hidden, c.hidden, next, (int)has_next));
+  return LSK_OK;
+}
+
+// Adaptive batched round (lsk_round_batch_adaptive): the rows of enqueue_round_batch(E, B, d) with the
+// conditional bodies of enqueue_round_adaptive.  Body j holds step j's head and tokens for every
+// sequence, the confidence kernel, then layers < E of row j + 1 of every sequence; it runs iff some
+// active sequence is still drafting after step j - 1.  Step 0 and row 1's layers always run.  The
+// accept keeps min(d_seq[s], the step sequence s stopped at) drafts: conf_seqs->d_stop.
+static int enqueue_round_batch_adaptive(lsk_engine* e, int E, int B, int d) {
+  const lsk_config& c = e->cfg;
+  const int* len = &e->bstate->len;
+  const BatchRows rows = batch_rows(e, B, d);
+  std::vector<cudaGraphConditionalHandle> cond(d, 0);
+  if (e->use_graph) {
+    cudaStreamCaptureStatus cs;
+    cudaGraph_t graph = nullptr;
+    CU(cudaStreamGetCaptureInfo(e->stream, &cs, nullptr, &graph, nullptr, nullptr));
+    for (int j = 1; j < d; ++j) CU(cudaGraphConditionalHandleCreate(&cond[j], graph, 0, cudaGraphCondAssignDefault));
+  }
+  const bool graph = e->use_graph;
+  e->cur_class = CLS_MISC;
+  CU(launch(e, embed_seq_tokens_kernel, dim3(B), dim3(256), 0, (const __nv_bfloat16*)e->embed, c.hidden,
+            (const DevState*)e->bstate, e->hidden, rows.stride));
+  for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, 0, B, len, 0, &rows.draft));
+  TRY(enqueue_draft_token_seqs(e, 0, B, d, rows.stride));
+  TRY(emit_draft_confidence_seqs(e, 0, B, d, graph && d > 1 ? cond[1] : 0, graph && d > 1));
+  for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, 1, B, len, 1, &rows.draft));
+  for (int j = 1; j < d; ++j) {
+    TRY(enqueue_if(e, cond[j], [&]() -> int {
+      TRY(enqueue_draft_token_seqs(e, j, B, d, rows.stride));
+      TRY(emit_draft_confidence_seqs(e, j, B, d, graph && j + 1 < d ? cond[j + 1] : 0, graph && j + 1 < d));
+      for (int l = 0; l < E; ++l) TRY(enqueue_layer(e, l, j + 1, B, len, j + 1, &rows.draft));
+      return LSK_OK;
+    }));
+  }
+  return enqueue_verify_seqs(e, E, B, d, rows, (const int*)e->conf_seqs->d_stop);
 }
 
 static int enqueue_ar(lsk_engine* e, int n_layers_run) {
@@ -1357,6 +1433,7 @@ static MemTable mem_table(const lsk_config& c, const EngineShape& s, int sm_coun
   t.batch_ctl = {(size_t)2 * kMaxRows * 4, S};
   t.batch_arrive = {(size_t)kMaxRows * s.kv_heads_l * 4, S};
   t.batch_seeds = {(size_t)kMaxRows * 8, S};
+  t.conf_seqs = {sizeof(ConfSeqsScratch), S};
   t.peer_region = {peer_region_layout(c.tp_size, c.hidden).total, S};
   return t;
 }
@@ -1408,6 +1485,7 @@ static void plan_memory(const lsk_config& c, const EngineShape& s, const MemTabl
   if (u.batch_seqs > 0)                                // sized for max_rows sequences, whatever the batch
     for (const MemBuf& b : {t.batch_state, t.batch_ctl, t.batch_arrive}) add(b, 1);
   if (u.batch_seqs > 0 && u.sampling) add(t.batch_seeds, 1);
+  if (u.batch_seqs > 0 && u.adaptive) add(t.conf_seqs, 1);
 }
 
 static lsk_memory_plan plan_of(const int64_t* cat) {
@@ -1996,6 +2074,20 @@ int lsk_round(lsk_engine* e, int32_t d_req, lsk_round_out* out) {
   return LSK_OK;
 }
 
+// What every adaptive round needs before its first launch: the stream conditional bodies are captured
+// on (graph mode; driver >= 12.4), draft_confidence_kernel's scratch, and the logits rows greedy drafts
+// materialise.
+static int prepare_adaptive(lsk_engine* e) {
+  if (e->use_graph && !e->body_stream) {
+    int drv = 0;
+    CU(cudaDriverGetVersion(&drv));
+    if (drv < 12040) return fail(LSK_ERR_CUDA, "adaptive rounds need CUDA graph conditional nodes (driver >= 12.4, found %d)", drv);
+    CU(cudaStreamCreateWithFlags(&e->body_stream, cudaStreamNonBlocking));
+  }
+  TRY(alloc_once(e, &e->conf_scratch, e->sizes.conf_scratch, true));
+  return ensure_logits(e);
+}
+
 int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_round_out* out,
                        float* draft_conf_out) {
   if (!e || !out) return fail(LSK_ERR_INVALID, "null argument");
@@ -2008,14 +2100,7 @@ int lsk_round_adaptive(lsk_engine* e, int32_t d_max, float min_confidence, lsk_r
   if (E < 1 || E > e->cfg.n_layers) return fail(LSK_ERR_INVALID, "self-speculation needs 1 <= exit_layer <= n_layers (got %d)", E);
   if (e->host_len + d_max + 2 > e->max_pos) return fail(LSK_ERR_CTX, "context %d + %d exceeds max_ctx", e->host_len, d_max + 1);
   if (d_max == 0) return lsk_round(e, 0, out);      // no draft to stop: the reference's tail round
-  if (e->use_graph && !e->body_stream) {
-    int drv = 0;
-    CU(cudaDriverGetVersion(&drv));
-    if (drv < 12040) return fail(LSK_ERR_CUDA, "adaptive rounds need CUDA graph conditional nodes (driver >= 12.4, found %d)", drv);
-    CU(cudaStreamCreateWithFlags(&e->body_stream, cudaStreamNonBlocking));
-  }
-  TRY(alloc_once(e, &e->conf_scratch, e->sizes.conf_scratch, true));
-  TRY(ensure_logits(e));                  // greedy drafts materialise their logits row
+  TRY(prepare_adaptive(e));
   // the threshold is read from device memory: one graph per round shape serves every threshold
   CU(cudaMemcpyAsync(&e->state->min_conf, &min_confidence, sizeof(float), cudaMemcpyHostToDevice, e->stream));
   const long long key = ((long long)E << 20) | ((long long)d_max << 8) | (e->gen.sample ? 4 : 0) | 8 | 1 |
@@ -2139,16 +2224,16 @@ int lsk_prefill_batch_seeded(lsk_engine* e, const int32_t* ids, const int32_t* o
   return prefill_batch(e, ids, offsets, n_seqs, seeds, slot_positions_out);
 }
 
-int lsk_round_batch(lsk_engine* e, int32_t d_req, const int32_t* d_seq, const int32_t* active,
-                    lsk_round_out* outs) {
-  if (!e || !outs) return fail(LSK_ERR_INVALID, "null argument");
-  if (!e->batch_n) return fail(LSK_ERR_STATE, "lsk_prefill_batch must precede lsk_round_batch");
+// lsk_round_batch's and lsk_round_batch_adaptive's preconditions; fills ctl with the round's d_seq and
+// active flags ([2][kMaxRows], batch_ctl's layout).
+static int check_batch_round(lsk_engine* e, const char* fn, int32_t d_req, const int32_t* d_seq,
+                             const int32_t* active, int* ctl) {
+  if (!e->batch_n) return fail(LSK_ERR_STATE, "lsk_prefill_batch must precede %s", fn);
   TRY(check_batch_generation(e, e->batch_seeded));
-  const int B = e->batch_n, E = e->gen.exit_layer;
+  const int B = e->batch_n;
   if (d_req < 0 || B * (d_req + 1) > e->max_rows)
     return fail(LSK_ERR_INVALID, "%d sequences x (d_req %d + 1) rows exceed the %d rows of a step", B, d_req,
                 e->max_rows);
-  int ctl[2 * kMaxRows] = {};
   for (int s = 0; s < B; ++s) {
     ctl[s] = d_seq ? d_seq[s] : d_req;
     ctl[kMaxRows + s] = active ? (active[s] != 0) : 1;
@@ -2160,14 +2245,55 @@ int lsk_round_batch(lsk_engine* e, int32_t d_req, const int32_t* d_seq, const in
     if (e->batch_len[s] + d_req + 2 > slot)
       return fail(LSK_ERR_CTX, "sequence %d: context %d + %d exceeds its slot of %d positions", s, e->batch_len[s],
                   d_req + 1, slot);
+  return LSK_OK;
+}
+
+static void copy_batch_results(lsk_engine* e, lsk_round_out* outs) {
+  for (int s = 0; s < e->batch_n; ++s) {
+    copy_result(e->bres_host[s], &outs[s]);
+    e->batch_len[s] = outs[s].kv_len;
+  }
+}
+
+int lsk_round_batch(lsk_engine* e, int32_t d_req, const int32_t* d_seq, const int32_t* active,
+                    lsk_round_out* outs) {
+  if (!e || !outs) return fail(LSK_ERR_INVALID, "null argument");
+  int ctl[2 * kMaxRows] = {};
+  TRY(check_batch_round(e, "lsk_round_batch", d_req, d_seq, active, ctl));
+  const int B = e->batch_n, E = e->gen.exit_layer;
   CU(cudaMemcpyAsync(e->batch_ctl, ctl, sizeof(ctl), cudaMemcpyHostToDevice, e->stream));
   const long long key = ((long long)E << 20) | ((long long)d_req << 8) | (e->gen.sample ? 4 : 0) | 16 | 1 |
                         ((long long)B << 40);
   TRY(run_cached(e, key, [&]() { return enqueue_round_batch(e, E, B, d_req); }));
-  for (int s = 0; s < B; ++s) {
-    copy_result(e->bres_host[s], &outs[s]);
-    e->batch_len[s] = outs[s].kv_len;
-  }
+  copy_batch_results(e, outs);
+  return LSK_OK;
+}
+
+int lsk_round_batch_adaptive(lsk_engine* e, int32_t d_max, const int32_t* d_seq, const int32_t* active,
+                             float min_confidence, lsk_round_out* outs, float* draft_conf_out) {
+  if (!e || !outs) return fail(LSK_ERR_INVALID, "null argument");
+  if (!(min_confidence >= 0.f && min_confidence <= 1.f))
+    return fail(LSK_ERR_INVALID, "min_confidence %g outside [0, 1]", (double)min_confidence);
+  int ctl[2 * kMaxRows] = {};
+  TRY(check_batch_round(e, "lsk_round_batch_adaptive", d_max, d_seq, active, ctl));
+  if (d_max == 0) return lsk_round_batch(e, 0, d_seq, active, outs);   // no draft to stop
+  const int B = e->batch_n, E = e->gen.exit_layer;
+  TRY(prepare_adaptive(e));
+  TRY(alloc_once(e, &e->conf_seqs, e->sizes.conf_seqs, true));
+  CU(cudaMemcpyAsync(e->batch_ctl, ctl, sizeof(ctl), cudaMemcpyHostToDevice, e->stream));
+  // the threshold is read from device memory: one graph per round shape serves every threshold
+  CU(cudaMemcpyAsync(&e->conf_seqs->min_conf, &min_confidence, sizeof(float), cudaMemcpyHostToDevice, e->stream));
+  const long long key = ((long long)E << 20) | ((long long)d_max << 8) | (e->gen.sample ? 4 : 0) | 16 | 8 | 1 |
+                        ((long long)B << 40);
+  e->adaptive = true;
+  const int st = run_cached(e, key, [&]() { return enqueue_round_batch_adaptive(e, E, B, d_max); });
+  e->adaptive = false;
+  e->pdl_break = false;
+  TRY(st);
+  copy_batch_results(e, outs);
+  if (draft_conf_out)
+    for (int s = 0; s < B; ++s)
+      for (int i = 0; i < outs[s].n_drafted; ++i) draft_conf_out[(size_t)s * LSK_MAX_SPEC + i] = e->bres_host[s].conf[i];
   return LSK_OK;
 }
 

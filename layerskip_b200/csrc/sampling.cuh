@@ -643,4 +643,108 @@ draft_confidence_kernel(const float* __restrict__ logits, const float* __restric
   if (has_next) cudaGraphSetConditional(next, stop ? 0u : 1u);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Confidence-threshold drafting for a batch (lsk_round_batch_adaptive).  Draft step j of sequence
+// s = blockIdx.y: the confidence of its draft row and the solo stop rule, with d_seq[s] for d_max,
+// into st[s] and d_stop[s] (what the batched accept kernels take as their d_seq).  Sequence s drafts
+// at step j iff it is active and j < its d_stop (j < d_seq[s] at step 0); a sequence that stopped
+// still has its rows computed while others draft on, but its d_stop and confidences stay as they
+// were.  Draft step j + 1 runs iff some active sequence has d_stop > j + 1: the last sequence to be
+// decided sets the conditional (an OR over the final d_stop values, so the vote does not depend on
+// timing).  Greedy confidences partition, walk and merge the columns exactly as
+// draft_confidence_kernel (grid.x = its grid), so they are bit-identical to a solo round's; sampled
+// ones read probs row s * seq_rows + j (grid.x = 1).  Step 0 zeroes hidden rows 2 .. d of every
+// sequence (rows s * seq_rows + 2 .., d = seq_rows - 1), for the reason draft_confidence_kernel
+// gives.  The body restates draft_confidence_kernel's rather than sharing it, which would change
+// that kernel's instructions.
+// ---------------------------------------------------------------------------------------------
+struct ConfSeqsScratch {
+  float m[kMaxRows][kConfMaxCtas], s[kMaxRows][kConfMaxCtas];
+  unsigned int arrive[kMaxRows];         // column slices of sequence s merged in this launch
+  unsigned int decided;                  // sequences decided in this launch
+  int d_stop[kMaxRows];                  // drafts sequence s keeps (seeded from d_seq at step 0)
+  float min_conf;                        // the batch's threshold, set by the host before each round
+};
+
+__global__ void __launch_bounds__(kConfThreads)
+draft_confidence_seqs_kernel(const float* __restrict__ logits, int ld, const float* __restrict__ probs, int V,
+                             int seq_rows, DevState* __restrict__ sts, const GenParams* __restrict__ gpp,
+                             RoundResult* __restrict__ ress, ConfSeqsScratch* __restrict__ cs,
+                             const int* __restrict__ d_seq, const int* __restrict__ active, int j,
+                             float* __restrict__ hidden, int hidden_ld, cudaGraphConditionalHandle next,
+                             int has_next) {
+  __shared__ float s_m[kConfThreads / 32], s_s[kConfThreads / 32];
+  __shared__ int s_last;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int q = blockIdx.y;
+  if (j == 0) {
+    const int n4 = (seq_rows - 2) * (hidden_ld >> 2);
+    float4* dst = reinterpret_cast<float4*>(hidden + ((size_t)q * seq_rows + 2) * hidden_ld);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x)
+      dst[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  DevState* st = &sts[q];
+  float conf;
+  if (logits != nullptr) {
+    const float* row = logits + (size_t)q * ld;
+    const int per = (V + gridDim.x - 1) / gridDim.x;
+    const int lo = blockIdx.x * per, hi = min(V, lo + per);
+    float m = -INFINITY, s = 0.f;
+    for (int c = lo + threadIdx.x; c < hi; c += kConfThreads) {
+      const float v = row[c];
+      if (v == -INFINITY) continue;
+      if (v > m) { s = s * expf(m - v) + 1.f; m = v; }
+      else s += expf(v - m);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float om = __shfl_xor_sync(0xffffffffu, m, o), os = __shfl_xor_sync(0xffffffffu, s, o);
+      lse_merge(m, s, om, os);
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) { s_m[warp] = m; s_s[warp] = s; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int w = 1; w < kConfThreads / 32; ++w) lse_merge(m, s, s_m[w], s_s[w]);
+      cs->m[q][blockIdx.x] = m;
+      cs->s[q][blockIdx.x] = s;
+      __threadfence();
+      s_last = atomicAdd(&cs->arrive[q], 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last || threadIdx.x != 0) return;
+    __threadfence();
+    m = __ldcg(&cs->m[q][0]);
+    s = __ldcg(&cs->s[q][0]);
+    for (int b = 1; b < gridDim.x; ++b) lse_merge(m, s, __ldcg(&cs->m[q][b]), __ldcg(&cs->s[q][b]));
+    cs->arrive[q] = 0;
+    conf = 1.0f / s;
+  } else {
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    conf = probs[((size_t)q * seq_rows + j) * V + st->tok[1 + j]];
+  }
+  // one thread per sequence from here on
+  const int d_lim = d_seq[q];
+  const int prev = j == 0 ? d_lim : cs->d_stop[q];
+  if (active[q] && j < prev) {
+    const GenParams gp = *gpp;
+    st->conf[j] = conf;
+    ress[q].conf[j] = conf;              // the sampled accept does not copy confidences
+    const bool stop = j + 1 == d_lim || is_eos(gp, st->tok[1 + j]) || conf < cs->min_conf;
+    st->d_stop = cs->d_stop[q] = stop ? j + 1 : d_lim;
+  } else if (j == 0) {
+    st->d_stop = cs->d_stop[q] = prev;
+  }
+  __threadfence();
+  if (atomicAdd(&cs->decided, 1u) != gridDim.y - 1) return;
+  __threadfence();
+  cs->decided = 0;
+  if (!has_next) return;
+  unsigned int go = 0;
+  for (int r = 0; r < (int)gridDim.y; ++r)
+    if (active[r] && __ldcg(&cs->d_stop[r]) > j + 1) go = 1u;
+  cudaGraphSetConditional(next, go);
+}
+
 }  // namespace lsk

@@ -249,15 +249,44 @@ class Engine:
         `round(d_seq[s])` of that sequence alone would.  An inactive sequence commits nothing and gets
         an empty RoundOutput (no tokens, kv_len unchanged)."""
         n = self._batch_n
+        ds, act = self._batch_ctl(d_seq, active)
+        outs = (_lib.lsk_round_out * (_lib.LSK_MAX_SPEC + 1))()    # up to max_rows sequences
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_round_batch(self._h, int(d_req), ds, act, outs))
+        return [self._round_output(o) for o in outs[:n]]
+
+    def round_batch_adaptive(self, d_max: int, min_confidence: float, d_seq: Optional[Sequence[int]] = None,
+                             active: Optional[Sequence[bool]] = None) -> List[RoundOutput]:
+        """`round_batch(d_max, d_seq, active)` with `round_adaptive`'s stop rule for every sequence:
+        sequence s stops drafting after its first draft that is an EOS or whose confidence is below
+        `min_confidence`, or after d_seq[s] drafts, and a draft step runs only while some active
+        sequence is still drafting.  Each active sequence's output is bit-identical to
+        `round_adaptive(d_seq[s], min_confidence)` of that sequence alone, `draft_confidence` included;
+        an inactive one gets an empty RoundOutput."""
+        n = self._batch_n
+        ds, act = self._batch_ctl(d_seq, active)
+        outs = (_lib.lsk_round_out * (_lib.LSK_MAX_SPEC + 1))()
+        conf = (C.c_float * ((_lib.LSK_MAX_SPEC + 1) * _lib.LSK_MAX_SPEC))()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.lsk_round_batch_adaptive(self._h, int(d_max), ds, act, float(min_confidence),
+                                                          outs, conf))
+        res = []
+        for s, o in enumerate(outs[:n]):
+            r = self._round_output(o)
+            base = s * _lib.LSK_MAX_SPEC
+            r.draft_confidence = [float(x) for x in conf[base:base + o.n_drafted]]
+            res.append(r)
+        return res
+
+    def _batch_ctl(self, d_seq, active):
+        """round_batch's d_seq and active flags as C arrays (None stays None: the library's default)."""
+        n = self._batch_n
         for name, v in (("d_seq", d_seq), ("active", active)):
             if v is not None and len(v) != n:
                 raise ValueError(f"{name} has {len(v)} entries for a batch of {n} sequences")
         ds = (C.c_int32 * n)(*[int(x) for x in d_seq]) if d_seq is not None else None
         act = (C.c_int32 * n)(*[int(bool(x)) for x in active]) if active is not None else None
-        outs = (_lib.lsk_round_out * (_lib.LSK_MAX_SPEC + 1))()    # up to max_rows sequences
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.lsk_round_batch(self._h, int(d_req), ds, act, outs))
-        return [self._round_output(o) for o in outs[:n]]
+        return ds, act
 
     KERNEL_CLASSES = ("qkv", "attention", "o_proj", "gate_up", "down", "lm_head", "small", "comm")
 

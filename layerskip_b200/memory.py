@@ -28,7 +28,8 @@ def plan_memory(arch: LlamaArch, max_ctx: int = 4096, tp_size: int = 1, sampling
     `ngram_ban` a `begin` with sampling / the n-gram ban, `adaptive` a `round_adaptive`, `scoring`
     an `lsk_score`, `score_exits` = k an `lsk_score_exits` with k exits (`score_exits_sampled`: with
     acceptance probabilities), `batch_scoring` an `lsk_score_batch` or `lsk_score_prefixed`,
-    `batch_seqs` > 0 an `lsk_prefill_batch` of up to that many sequences (the same buffers for any count).  With
+    `batch_seqs` > 0 an `lsk_prefill_batch` of up to that many sequences (the same buffers for any count;
+    with `adaptive`, also `round_batch_adaptive`'s confidence scratch).  With
     tp_size > 1 the peer region of the one-shot collectives is counted."""
     cfg = arch.lsk_config(max_ctx, tp_size=tp_size,
                           flags=(_lib.LSK_FLAG_KEEP_LOGITS if keep_logits else 0) |
